@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
 """bench.py -- proof-gen seconds for the guest-keccak APC segment shape (2^20 rows x 2022 columns, 187 constraints of
-degree <= 3, 1734 bus interactions: /root/reference/openvm-riscv/src/lib.rs:1377-1386) on N B200s, through the C ABI of
+degree <= 3, 1734 bus interactions: openvm-riscv/src/lib.rs:1377-1386 of powdr) on N H100s, through the C ABI of
 include/powdr_b200.h.
 
   python bench.py --gpus N --steps K --warmup W                 # native CUDA arm (torchrun launches N ranks for N > 1)
@@ -10,8 +10,12 @@ One step = one segment per GPU through the whole path: main trace commit (LDE + 
 (generate, LDE, commit) -> quotient -> quotient commit -> openings at zeta / zeta*w -> FRI commit phase -> proof of work (16 bits)
 -> 100 queries.  `value` = device-timed seconds per segment with the trace already resident in HBM (max over ranks, divided by
 the N segments proved concurrently); `e2e` = the same through pb_prove_segment + pb_query_segment with the trace in pinned
-HOST memory (H2D inside the timed region, proof and query openings read back).  Inputs (8.5 GB/segment) exceed the 126 MB
+HOST memory (H2D inside the timed region, proof and query openings read back).  Inputs (8.5 GB/segment) exceed the 50 MB
 L2, so no L2 flush is needed between iterations.  torch is plumbing only: device memory, the stream, events, NCCL.
+
+  --dump-outputs DIR   after the timed steps, writes what the last timed step returned (the proof's fields and the query
+                       openings of pb_query_segment) as DIR/<name>.npy, float64 (every value is a u32 field word, exact);
+                       the inputs are seeded, so two builds can be compared output for output.
 """
 import argparse
 import math
@@ -27,6 +31,9 @@ sys.path.insert(0, ROOT)
 
 METRIC = "proof-gen sec for guest-keccak APC segment @2^20 rows"
 P = 2013265921
+H100_HBM_GBS = 3350.0             # H100 SXM data sheet; a measured MEASURED_PEAKS.json["hbm_gbs"] takes precedence
+H100_MAX_SM_MHZ = 1980.0          # H100 SXM maximum SM clock, when nvidia-smi gives no sample
+H100_MULMOD_PER_CLK_SM = 12.5     # signed Montgomery products per clock per SM, scripts/microbench.cu on an H100 SXM
 
 
 def parse():
@@ -46,6 +53,8 @@ def parse():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--metrics-out", default="", help="write the last step's stage times as an OpenVM-1 metrics JSON (basic_metrics.py schema)")
     ap.add_argument("--no-e2e", action="store_true")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write the last timed step's proof and query openings as DIR/<name>.npy (float64)")
     ap.add_argument("--no-sharded", action="store_true", help="skip the one-segment-on-all-GPUs (strong scaling) measurement at N > 1")
     ap.add_argument("--one-transcript", action="store_true",
                     help="multichip workload: prove all 50 chips under ONE transcript on one GPU (pb_prove_chips) instead of one proof per chip")
@@ -74,7 +83,7 @@ def machine_for(a):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index):
         self.rows, self.proc, self.index = [], None, index
@@ -216,6 +225,17 @@ def run_reference(a):
         "cpu_baseline": base, "e2e": {"value": v, "unit": "s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}}))
 
 
+def dump_outputs(out_dir, proof, queries, ys):
+    """one .npy per proof field (proof_<field>) plus the query openings and the opened values, float64: every value is a
+    canonical u32 field word, which float64 holds exactly"""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"proof_" + k: v for k, v in proof.items()}
+    arrays["queries"], arrays["opened_values"] = queries, ys
+    for name, v in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), np.asarray(v, dtype=np.float64))
+
+
 def run_native(a):
     import numpy as np
     import torch
@@ -254,11 +274,11 @@ def run_native(a):
 
     def step_device():
         proof = ctx.prove_segment(air, trace.data_ptr(), a.log_n, w, on_device=True)
-        ctx.query_segment(a.log_n, w, wp)                     # query phase: 100 openings gathered on the device, read back
+        openings = ctx.query_segment(a.log_n, w, wp)          # query phase: 100 openings gathered on the device, read back
         if world > 1:   # the path's one exchange: all-gather of the segment commitments (Merkle caps) over NCCL/NVLink
             caps.copy_(torch.tensor(proof["trace_root"] + proof["quotient_root"], dtype=torch.int64).to(torch.int32), non_blocking=True)
             parallel.all_gather_caps(caps.view(2, 8), dist)
-        return proof
+        return proof, openings
 
     def sync_all():
         torch.cuda.synchronize()
@@ -279,10 +299,12 @@ def run_native(a):
     sampler.mark()
     e0.record(stream)
     for _ in range(a.steps):
-        proof = step_device()
+        proof, (queries, ys) = step_device()
     e1.record(stream)
     sync_all()
     ms = e0.elapsed_time(e1)
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, proof, queries, ys)
     clocks = sampler.stop() if rank == 0 else None
     launches = ctx.launch_count() - launches0
     n_leaf, leaf_ms, leaf_bytes = ctx.leaf_kernel_profile()
@@ -332,15 +354,9 @@ def run_native(a):
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        peak = float(peaks.get("hbm_gbs", 6650.0))
+        peak = float(peaks.get("hbm_gbs", H100_HBM_GBS))
         achieved = (leaf_bytes / 1e9) / (leaf_ms / 1e3) if leaf_ms > 0 else 0.0
-        traffic = None
-        try:
-            # one `ncu --set full` capture of this kernel gives DRAM bytes / algorithmic bytes of a launch; the timed launches differ in
-            # width (main, permutation, quotient matrices), so the ratio is applied to their average algorithmic size
-            traffic = json.load(open(os.path.join(ROOT, "profiles", "leaf_kernel_traffic.json")))["dram_over_algorithmic"] * leaf_bytes / max(1, n_leaf)
-        except Exception:
-            pass
+        n_sms = torch.cuda.get_device_properties(dev).multi_processor_count
         nn, ww, wpp = float(n), float(w), float(wp)
         alg = {"lde": 12 * nn * ww, "merkle": 8 * nn * ww + 64 * nn, "quotient": 8 * nn * (ww + (2 * wpp if wp else 0)) + 32 * nn,
                "logup_gen": 4 * nn * (ww + wpp), "logup_commit": 12 * nn * wpp + 8 * nn * wpp + 64 * nn}
@@ -353,17 +369,17 @@ def run_native(a):
                        "parallelism": "1 segment per GPU, NCCL all-gather of Merkle caps" if world > 1 else "single GPU"},
             "gpu_launches": launches, "clocks": clocks,
             "roofline": {"bound": "hbm", "kernel": "p2::leaf_hash_cols_kernel (Poseidon2 leaf hashing)", "achieved": achieved, "peak": peak,
-                         "unit": "GB/s", "frac": achieved / peak, "traffic": traffic, "launches_timed": n_leaf,
-                         "avg_launch_ms": leaf_ms / max(1, n_leaf), "peak_source": "MEASURED_PEAKS.json" if peaks else "fallback",
+                         "unit": "GB/s", "frac": achieved / peak, "launches_timed": n_leaf,
+                         "avg_launch_ms": leaf_ms / max(1, n_leaf), "peak_source": "MEASURED_PEAKS.json" if peaks else "H100 SXM data sheet",
                          "note": "integer-ALU-bound kernel (~22 mulmod per byte); HBM fraction is reported as the contract asks"},
             # the same kernel against the roof that actually binds it: the integer multiplier pipe.  One Poseidon2 permutation
             # is 564 Montgomery products (10 pipe cycles each) + 117 constant products (8 cycles) = 657.6 Montgomery-product
-            # equivalents; peak = 12.6 products/clk/SM measured by scripts/microbench.cu (profiles/r01_microbench.txt)
+            # equivalents; peak = H100_MULMOD_PER_CLK_SM products/clk/SM (scripts/microbench.cu)
             "roofline_integer": (lambda perms, peak_i: {"bound": "imad pipe", "achieved": perms * 657.6 / (leaf_ms / 1e3) / 1e12 if leaf_ms > 0 else 0.0,
                                                         "peak": peak_i / 1e12, "unit": "T mulmod/s",
                                                         "frac": (perms * 657.6 / (leaf_ms / 1e3)) / peak_i if leaf_ms > 0 else 0.0})(
                 (leaf_bytes / (4.0 * ww + 32.0)) * math.ceil(ww / 8.0) if n_leaf else 0.0,
-                12.6 * 148 * ((clocks or {}).get("sm_mhz") or 1965.0) * 1e6),
+                H100_MULMOD_PER_CLK_SM * n_sms * ((clocks or {}).get("sm_mhz") or H100_MAX_SM_MHZ) * 1e6),
             "stages_ms": stage_ms, "keygen_s": keygen_s, "perm_width": wp,
             "stage_roofline_frac": {k: (alg[k] / 1e9) / (stage_ms[k] / 1e3) / peak for k in alg if stage_ms.get(k, 0) > 0},
             "segments_per_s": world / (ms_per_step / 1e3),
@@ -684,7 +700,7 @@ def run_stage0(a):
         ctx.prove_segment(air, out.data_ptr(), a.log_n, W, on_device=True)
         ctx.query_segment(a.log_n, W, air.perm_width)
     w_ms = timed(whole, max(1, a.steps // 2))
-    peak = 6575.1
+    peak = H100_HBM_GBS
     try:
         peak = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"])
     except Exception:
@@ -772,7 +788,7 @@ def run_pairing(a):
     same = bool((lo == hi).all().item())
     if rank == 0:
         print(json.dumps({
-            "metric": "proof-gen sec for ONE wide APC segment (guest-pairing shape) column-sharded over N B200", "value": float(t.item()), "unit": "s",
+            "metric": "proof-gen sec for ONE wide APC segment (guest-pairing shape) column-sharded over N GPUs","value": float(t.item()), "unit": "s",
             "n_gpus": world, "steps": a.steps, "warmup": a.warmup, "ms_per_step": float(t.item()) * 1e3, "higher_is_better": False, "scaling": "strong",
             "vs_baseline": None, "dtype": "u32 (BabyBear, Montgomery)", "data": "synthetic",
             "config": {"workload": "2^%d rows x %d cols, %d constraints deg<=3, no bus interactions (sharded prover), log_blowup 1; trace %.1f GB, LDE %.1f GB "
@@ -788,6 +804,8 @@ def run_pairing(a):
 
 if __name__ == "__main__":
     args = parse()
+    if args.dump_outputs and (args.impl != "native" or args.workload != "keccak"):
+        raise SystemExit("--dump-outputs writes the outputs of the native keccak workload only")
     if args.impl == "reference":
         run_reference(args)
     elif args.workload == "multichip":

@@ -1,5 +1,5 @@
 /*
- * powdr_b200 -- C ABI of the B200-native STARK proving hot path for powdr autoprecompile (APC) chips over BabyBear.
+ * powdr_b200 -- C ABI of the H100-native STARK proving hot path for powdr autoprecompile (APC) chips over BabyBear.
  *
  * Conventions (copied from the reference's only in-tree FFI, /root/reference/openvm/src/cuda_abi.rs:8-64):
  *   - every entry point returns int: 0 = ok, a positive cudaError_t, or a negative PB_ERR_* code; nothing aborts;
@@ -77,7 +77,7 @@ int pb_air_free(pb_air_t* air);
  * provers (e.g. one per GPU) compile their own handle, which is also what binds the kernels to their device's CUDA context. */
 /* 1 when the AIR runs on its NVRTC-generated straight-line kernel, 0 when on the bytecode interpreter kernel */
 int pb_air_is_jit(const pb_air_t* air);
-/* host-only check of the code generator: packs the program, generates CUDA C and compiles it for sm_100a (no device needed) */
+/* host-only check of the code generator: packs the program, generates CUDA C and compiles it for sm_90a (no device needed) */
 int pb_air_jit_compile_only(const uint32_t* bytecode, size_t n_words, const pb_expr_span_t* constraints, size_t n_constraints,
                             uint32_t width, size_t* cubin_bytes);
 /* d_quotient: [2 chunks][4 limbs][2^log_n], chunk = parity of the natural LDE index (= top bit of the bit-reversed row),
@@ -258,7 +258,7 @@ typedef struct { uint32_t bus_id; uint32_t num_args; uint32_t args_index_off; } 
  * Attaches the bus interactions PowdrAir::eval pushes (/root/reference/openvm/src/powdr_extension/chip.rs:117-128) to a compiled
  * AIR, in the layout compile_bus_to_gpu produces (cuda/mod.rs:143-177: per interaction the spans [mult, arg_0 .. arg_{k-1}]
  * from args_index_off) with the PUSH_APC operand being the COLUMN INDEX.  Generates and compiles the AIR's LogUp kernels
- * (NVRTC, sm_100a); pb_prove_segment then runs the permutation-trace phase for this AIR.  HOST pointers. */
+ * (NVRTC, sm_90a); pb_prove_segment then runs the permutation-trace phase for this AIR.  HOST pointers. */
 int pb_air_set_interactions(pb_ctx_t* ctx, pb_air_t* air, const uint32_t* bytecode, size_t n_words, const ExprSpan* arg_spans,
                             size_t n_arg_spans, const DevInteraction* interactions, size_t n_interactions);
 /* host-only check of the LogUp code generator (no device needed): generates and compiles the kernels, reports their size */

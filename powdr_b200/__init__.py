@@ -1,6 +1,6 @@
-"""powdr_b200 -- B200-native STARK proving hot path for powdr autoprecompile (APC) chips over BabyBear.
+"""powdr_b200 -- H100-native STARK proving hot path for powdr autoprecompile (APC) chips over BabyBear.
 
-The product is the sm_100a shared library behind include/powdr_b200.h; this package is the thin host-side mirror of the
+The product is the sm_90a shared library behind include/powdr_b200.h; this package is the thin host-side mirror of the
 reference's Rust call sites (machine JSON -> bytecode, launch wrappers, segment proving).  There is no CPU fallback:
 importing works anywhere, but every compute call needs the CUDA library and a GPU.
 """

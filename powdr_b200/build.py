@@ -1,4 +1,4 @@
-"""Build the sm_100a shared library in-tree (powdr_b200/_lib/libpowdr_b200.so) with nvcc.
+"""Build the sm_90a shared library in-tree (powdr_b200/_lib/libpowdr_b200.so) with nvcc.
 
 One CUDA translation unit (csrc/capi.cu) plus the host-only transcript permutation (csrc/transcript_host.cpp, g++) -> one .so
 exporting the C ABI of include/powdr_b200.h.  Cross-compiles without a GPU.
@@ -13,7 +13,7 @@ LIB_DIR = os.path.join(HERE, "_lib")
 LIB = os.path.join(LIB_DIR, "libpowdr_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 CXX = os.environ.get("CXX", "/usr/bin/g++")
-FLAGS = ["-std=c++17", "-O3", "-ldl", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+FLAGS = ["-std=c++17", "-O3", "-ldl", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
          "-Xcompiler", "-fPIC", "-shared", "-ccbin", "/usr/bin/g++"]
 
 

@@ -97,13 +97,13 @@ _lib = None
 
 
 def load_library(path=None):
-    """dlopen the in-tree sm_100a library; never falls back to anything else."""
+    """dlopen the in-tree sm_90a library; never falls back to anything else."""
     global _lib
     if _lib is not None:
         return _lib
     path = path or LIB_PATH
     if not os.path.exists(path):
-        raise LibraryMissing("%s not built: run `python -m powdr_b200.build` (nvcc, sm_100a)" % path)
+        raise LibraryMissing("%s not built: run `python -m powdr_b200.build` (nvcc, sm_90a)" % path)
     lib = C.CDLL(path)
     for name in EXPORTS:
         if not hasattr(lib, name):

@@ -2,7 +2,7 @@
 // (ncu r01: 143 k instructions per LDE row for the keccak-shaped AIR, 20 % of the HBM roof).  An autoprecompile's constraint
 // set is fixed at key-generation time, so pb_air_compile turns the packed program into straight-line CUDA C -- one SSA value
 // per node, constants folded into Shoup products, constraints grouped into small __noinline__ functions to keep ptxas
-// basic blocks short -- and compiles it with NVRTC for sm_100a.  NVRTC and the driver API are dlopen'ed lazily so the
+// basic blocks short -- and compiles it with NVRTC for sm_90a.  NVRTC and the driver API are dlopen'ed lazily so the
 // library itself links against nothing but cudart; when either is missing, or PB_AIR_NO_JIT is set, the interpreter
 // kernel (still CUDA) is used instead.
 #pragma once
@@ -245,7 +245,7 @@ inline std::string cache_path(const std::string& src) {
     uint64_t h1 = 1469598103934665603ull, h2 = 0x9e3779b97f4a7c15ull;
     for (unsigned char c : src) { h1 = (h1 ^ c) * 1099511628211ull; h2 = (h2 + c) * 0xff51afd7ed558ccdull; h2 ^= h2 >> 29; }
     char name[96];
-    snprintf(name, sizeof name, "/sm100a_%016llx%016llx_%zu.cubin", (unsigned long long)h1, (unsigned long long)h2, src.size());
+    snprintf(name, sizeof name, "/sm90a_%016llx%016llx_%zu.cubin", (unsigned long long)h1, (unsigned long long)h2, src.size());
     return d + name;
 }
 
@@ -265,7 +265,7 @@ inline int compile_chunk(const std::string& src, std::vector<char>& cubin) {
     Api& a = api();
     nvrtcProgram prog;
     if (a.CreateProgram(&prog, src.c_str(), "pb_air.cu", 0, nullptr, nullptr) != NVRTC_SUCCESS) return 4;
-    const char* opts[] = {"--gpu-architecture=sm_100a", "-std=c++17", "-lineinfo"};
+    const char* opts[] = {"--gpu-architecture=sm_90a", "-std=c++17", "-lineinfo"};
     nvrtcResult rc = a.CompileProgram(prog, 3, opts);
     if (rc != NVRTC_SUCCESS) {
         if (getenv("PB_AIR_JIT_VERBOSE")) {

@@ -3,7 +3,7 @@
 // (/root/reference/openvm/cuda/src/expr_eval.cuh:49-50: PUSH_CONST passes a canonical u32 through Fp(u)).
 // Everything on the device stays in this form; conversions happen only at the C-ABI edge.
 //
-// Montgomery product as two wide multiply-adds (sm_100a: IMAD.WIDE x2 + IMAD):
+// Montgomery product as two wide multiply-adds (sm_90a: IMAD.WIDE x2 + IMAD):
 //   t = a*b;  m = lo(t) * (-p^-1 mod 2^32);  d = m*p + t  (low word == 0);  r = hi(d) in [0, 2p)
 #pragma once
 #include <stdint.h>

@@ -145,6 +145,7 @@ struct McChip {
 
 struct pb_ctx {
     int device = 0;
+    int n_sms = 1;                    // multiprocessor count of `device` (sizes the LDE column batches)
     cudaStream_t stream = nullptr;
     uint64_t launches = 0;
     P2Host p2;
@@ -311,10 +312,8 @@ int get_fold_table(pb_ctx* ctx, int log_len) {
 
 // Merkle layers above the leaves: node-major, layer k+1 follows layer k.  Levels with more than MERKLE_COOP nodes are throughput
 // work: compress_block_kernel, one thread per permutation, up to 10 levels per launch.  Below that every level is ONE permutation
-// latency however few nodes it has (measured ~8.5 us per level one-thread-per-permutation, ~6 us with 16 lanes per permutation), so
-// they run on compress_coop_kernel: 128-node subtrees per CTA, then the last <= 128 nodes in one CTA.  Measured on B200
-// (profiles/README.md round 2c): a 2^12-row chip's FRI phase 1.07 -> 0.77 ms; with the threshold at 8192 nodes the 16-lane form
-// loses to the throughput form on the wider levels (keccak FRI phase 3.6 -> 4.6 ms), hence 1024.
+// latency however few nodes it has, and 16 lanes per permutation shorten that latency, so they run on compress_coop_kernel:
+// 128-node subtrees per CTA, then the last <= 128 nodes in one CTA.  On wider levels the one-thread-per-permutation form wins.
 constexpr size_t MERKLE_COOP = 1024;     // nodes
 constexpr size_t LEAF_COOP = 1024;       // rows: leaf sponges of shorter matrices run 16 lanes per row as well
 int merkle_upper(pb_ctx* ctx, uint32_t* d_layers, size_t log_h) {
@@ -360,6 +359,7 @@ int pb_ctx_create(pb_ctx_t** out, int device, void* cuda_stream) {
     ctx->stream = (cudaStream_t)cuda_stream;
     // any failure below releases what was created so far (pb_ctx_destroy tolerates a half-built context)
     auto init = [&]() -> int {
+        CK(cudaDeviceGetAttribute(&ctx->n_sms, cudaDevAttrMultiProcessorCount, device));
         for (auto& e : ctx->ev) CK(cudaEventCreate(&e));
         CK(cudaStreamCreateWithFlags(&ctx->copy_stream, cudaStreamNonBlocking));
         for (int i = 0; i < 2; i++) {
@@ -503,11 +503,10 @@ NttGeom make_geom(int n) {
 }
 
 // Column batch: the passes are integer-pipe bound (ncu: DRAM < 15 % busy), so filling the machine evenly matters more than
-// keeping the intermediates L2-resident.  Measured at 2^20: 4 columns -> 49.7 ms, 37 -> 35.5, 74 -> 34.5.
-// PB_LDE_BATCH overrides for experiments.
-size_t lde_column_batch(size_t N, size_t width) {
+// keeping the intermediates L2-resident: a batch is 16 tiles per SM.  PB_LDE_BATCH overrides for experiments.
+size_t lde_column_batch(const pb_ctx* ctx, size_t N, size_t width) {
     const size_t tiles_per_col = std::max<size_t>(1, N >> ntt::LOG_TILE_MAX);
-    size_t batch = std::max<size_t>(1, (size_t)148 * 16 / tiles_per_col);
+    size_t batch = std::max<size_t>(1, (size_t)ctx->n_sms * 16 / tiles_per_col);
     if (const char* e = getenv("PB_LDE_BATCH")) batch = std::max<size_t>(1, (size_t)atol(e));
     batch = std::min<size_t>(std::min<size_t>(batch, width), 32768);
     return (width + (width + batch - 1) / batch - 1) / ((width + batch - 1) / batch);     // equal-sized batches (no runt batch)
@@ -577,7 +576,7 @@ int pb_lde_batch(pb_ctx_t* ctx, const uint32_t* d_trace, size_t log_n, size_t wi
     int rc = get_twiddles(ctx, n, (int)log_blowup, shift, &tw);
     if (rc) return rc;
     const NttGeom g = make_geom(n);
-    const size_t batch = lde_column_batch(N, width);
+    const size_t batch = lde_column_batch(ctx, N, width);
     // PB_LDE_STREAMS > 1 (experiment): small column batches round-robin over several streams, so the four passes of different
     // batches overlap and the intermediates of the batches in flight can stay in L2
     int n_streams = 1;
@@ -1107,7 +1106,7 @@ int _apc_apply_bus(const uint32_t* d_output, int num_apc_calls, const uint32_t* 
 // ---- stage 0, generated periphery kernel (bus_jit.cuh): same histograms as _apc_apply_bus, straight-line code per AIR ----
 int pb_bus_compile(pb_ctx_t* ctx, const uint32_t* bc, size_t n_words, const ExprSpan* arg_spans, size_t n_arg_spans, const DevInteraction* ints, size_t n_ints,
                    uint32_t width, uint32_t var_range_bus_id, uint32_t tuple2_bus_id, uint32_t bitwise_bus_id, pb_bus_t** out) {
-    // ctx == NULL && out == NULL: host-only check of the code generator (packs, generates, compiles for sm_100a; no device needed)
+    // ctx == NULL && out == NULL: host-only check of the code generator (packs, generates, compiles for sm_90a; no device needed)
     const bool compile_only = !ctx && !out;
     if ((!compile_only && (!ctx || !out)) || (!bc && n_words) || (!arg_spans && n_arg_spans) || (!ints && n_ints)) return PB_ERR_INVALID_ARG;
     std::vector<uint32_t> code, pool;

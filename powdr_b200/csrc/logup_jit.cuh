@@ -181,8 +181,8 @@ inline Val emit_expr(std::string& src, const std::vector<uint32_t>& code, air::S
 
 constexpr size_t GROUP_CHUNKS_MAX = 8;
 // tuning knobs of the generated kernels (experiments: PB_LOGUP_GROUP / PB_LOGUP_BLOCK / PB_LOGUP_MINB)
-// chunks per generated function: measured on B200 at 2^18 rows x 1734 interactions (profiles/README.md): permutation kernel best at 2
-// (one inversion per 2 chunks), fold kernel at 1 -- fewer live Ext4 values beat the amortised inversion
+// chunks per generated function: permutation kernel 2 (one inversion per 2 chunks), fold kernel 1 -- fewer live Ext4 values beat
+// the amortised inversion
 inline size_t group_chunks(bool for_perm) {
     if (const char* e = getenv(for_perm ? "PB_LOGUP_GROUP_PERM" : "PB_LOGUP_GROUP_FOLD")) return std::min<size_t>(GROUP_CHUNKS_MAX, std::max<size_t>(1, (size_t)atol(e)));
     if (const char* e = getenv("PB_LOGUP_GROUP")) return std::min<size_t>(GROUP_CHUNKS_MAX, std::max<size_t>(1, (size_t)atol(e)));

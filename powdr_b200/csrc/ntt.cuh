@@ -2,7 +2,7 @@
 // (SURVEY.md §8 a6; call site main_trace_commit behind /root/reference/openvm-riscv/src/lib.rs:332).
 //
 // Per column:  evals over H (natural order)  --iNTT-->  coefficients  --coset NTT x 2^b-->  evals over shift*H',
-// rows bit-reversed.  B200 mapping:
+// rows bit-reversed.  H100 mapping:
 //   * inverse = decimation-in-frequency (natural in, bit-reversed coefficient slots out), forward = decimation-in-time
 //     on those slots (natural out): no standalone permutation pass; the one bit reversal is folded into the last store.
 //   * the coset shift is folded into the forward twiddles (w_u[k] = shift^(2^(n-1-u)) * omega^k), the 1/N into the last
@@ -12,11 +12,12 @@
 //       K2a inverse, bits [0,n_lo)   transposed tiles [2^n_lo rows x 32 lanes], lane = one contiguous 2^n_lo block
 //       K2b forward, bits [0,n_lo)   per coset, same geometry
 //       K3  forward, bits [n_lo,n)   per coset, strided tiles, then the bit-reversed store
-//     Each column crosses HBM once in (4N bytes) and once out (4N*2^b); intermediates are sized to stay in the 126 MB L2.
+//     Each column crosses HBM once in (4N bytes) and once out (4N*2^b); the batch is sized to fill the SMs, not to keep the
+//     intermediates in the 50 MB L2 (the passes are integer-pipe bound).
 //   * inside a pass the butterfly network never crosses lanes: a thread owns 2^q (q<=5) rows of one lane in REGISTERS and
 //     runs q radix-2 stages on them (80 butterflies per 32 loads + 32 stores for q=5); shared memory is touched once per
 //     round, conflict-free (lane = bank, XOR swizzle for the two transposed accesses).
-// Integer-pipe bound: a Montgomery product costs 10 FMA-pipe cycles per warp on sm_100 (IMAD.WIDE and IMAD.HI are half rate).
+// Integer-pipe bound: a Montgomery product costs 10 FMA-pipe cycles per warp on sm_90 (IMAD.WIDE and IMAD.HI are half rate).
 #pragma once
 #include "bb31.cuh"
 

@@ -60,7 +60,7 @@ __device__ __forceinline__ void external_linear(uint32_t (&s)[16]) {
 }
 
 // a * w mod p for a fixed w (Shoup): q = hi(a*w'), r = a*w - q*p in [0,2p), one correction.  IMAD.HI + 2 IMAD = 8 FMA-pipe
-// cycles per warp against 10 for a Montgomery product (IMAD.WIDE and IMAD.HI are half rate on sm_100), and no fix-up adds.
+// cycles per warp against 10 for a Montgomery product (IMAD.WIDE and IMAD.HI are half rate on sm_90), and no fix-up adds.
 __device__ __forceinline__ uint32_t mul_const(uint32_t a, uint32_t w, uint32_t wp) {
     const uint32_t q = __umulhi(a, wp);
     return bb::reduce_2p(a * w - q * bb::P);

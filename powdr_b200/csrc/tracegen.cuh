@@ -1,4 +1,4 @@
-// Stage 0: sm_100a re-designs of the reference's three APC trace-generation kernels, behind the SAME extern "C" entry
+// Stage 0: sm_90a re-designs of the reference's three APC trace-generation kernels, behind the SAME extern "C" entry
 // points and #[repr(C)] descriptors (/root/reference/openvm/src/cuda_abi.rs:8-95,150-169):
 //   _apc_tracegen            replaces apc_tracegen_kernel            (/root/reference/openvm/cuda/src/apc_tracegen.cu:35-66)
 //   _apc_apply_derived_expr  replaces apc_apply_derived_expr_kernel  (apc_tracegen.cu:72-100)

@@ -1,5 +1,5 @@
 // Integer-pipe micro-benchmarks that decide which roof binds the BabyBear kernels (SURVEY.md §7 step 0, App. D).
-// nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o microbench scripts/microbench.cu ; ./microbench
+// nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o microbench scripts/microbench.cu ; ./microbench
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>

@@ -1,7 +1,7 @@
-// Does the FP64 pipe of the B200 give the BabyBear kernels a second multiplier?  (sm_100a keeps full-rate FP64, unlike sm_103a.)
+// Does the FP64 pipe of the H100 give the BabyBear kernels a second multiplier?  (sm_90a has full-rate FP64.)
 // A modular product in doubles: h = a*b (rounded), l = fma(a,b,-h) (exact low part), q = rint(h/p), r = (h - q*p) + l: six
 // DP instructions, result in the symmetric range |r| <= 0.51 p for any |a|,|b| < 2^31.5, so products chain with no correction.
-// nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o microbench_fp64 scripts/microbench_fp64.cu ; ./microbench_fp64
+// nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o microbench_fp64 scripts/microbench_fp64.cu ; ./microbench_fp64
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>

@@ -7,11 +7,9 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
-REFERENCE = "/root/reference"
-
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with `-m gpu`)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with `-m gpu`)")
 
 
 @pytest.fixture(scope="session")

@@ -18,6 +18,8 @@ reference-derived fixtures and the oracle for the generated vectors):  python te
                                    single_div_nondet, wasm_register_reuse and keccak_apc_pre_opt (677 instructions, 27 521 cells): the
                                    REAL stage-0 gather pattern (the machines of the big fixture are not committed: 28 627 constraints)
   chips_mixed.json                 three chips of different heights under one transcript (orc_prove_chips): proof, cumulative sums, digests
+  v1_metrics_reference.json        an OpenVM-1 metrics file written by powdr_b200.metrics and what the reference's own
+                                   openvm-riscv/scripts/basic_metrics.py extracts from it (plots stubbed out: matplotlib is optional)
 """
 import glob
 import gzip
@@ -80,6 +82,7 @@ def main():
         with gzip.GzipFile(os.path.join(HERE, "stage0_subs.json.gz"), "wb", mtime=0) as f:
             f.write(json.dumps(st0, separators=(",", ":")).encode())
         print("wrote stage0_subs.json.gz", os.path.getsize(os.path.join(HERE, "stage0_subs.json.gz")), "bytes")
+        metrics_golden()
     rng = np.random.default_rng(2024)
     kat = {}
     kat["perm_zero"] = orc.poseidon2_permute(np.zeros(16, dtype=np.uint32)).tolist()
@@ -125,6 +128,32 @@ def main():
     proof, cs, ys, q = orc.prove_chips(chips, n_queries=g["n_queries"], pow_bits=g["pow_bits"])
     g.update(proof=proof, cumsums=cs.tolist(), ys_sha256=sha(ys), queries_sha256=sha(q))
     dump("chips_mixed.json", g)
+
+
+METRICS_STAGES_MS = {"h2d": 0.1, "lde": 34.0, "merkle": 130.0, "logup_gen": 46.0, "logup_commit": 270.0, "quotient": 60.0, "qlde": 0.3,
+                     "qmerkle": 1.3, "open": 25.0, "fri": 3.9, "pow": 0.3, "total": 571.0}
+
+
+def metrics_golden():
+    """the keccak-shaped metrics file of tests/test_host.py, read back by the reference's basic_metrics.extract_metrics"""
+    import tempfile
+    import types
+    from powdr_b200 import metrics
+    m = metrics.segment_metrics(METRICS_STAGES_MS, 1 << 20, 2022, 3348, 187, 1734, trace_gen_ms=12.0, query_ms=0.5)
+    with tempfile.TemporaryDirectory() as tmp:
+        path = os.path.join(tmp, "metrics.json")
+        metrics.write(path, m)
+        stub = {n: types.ModuleType(n) for n in ("matplotlib", "matplotlib.pyplot", "matplotlib.ticker")}
+        stub["matplotlib.ticker"].AutoMinorLocator = object
+        for n, mod in stub.items():
+            sys.modules.setdefault(n, mod)
+        sys.path.insert(0, os.path.join(REF, "openvm-riscv/scripts"))
+        import basic_metrics
+        out = basic_metrics.extract_metrics(path)
+        keys = ("num_segments", "powdr_ratio", "powdr_rows", "app_proof_time_excluding_trace_ms", "app_proof_cols", "app_proof_cells",
+                "app_proof_time_ms", "app_trace_gen_time_ms", "total_proof_time_ms", "total_proof_time_excluding_trace_ms")
+        dump("v1_metrics_reference.json", {"metrics_json": json.load(open(path)),
+                                           "extract_metrics": {k: (out[k].item() if hasattr(out[k], "item") else out[k]) for k in keys}})
 
 
 def chips_for(spec, seed):
