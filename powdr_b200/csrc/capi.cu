@@ -502,8 +502,10 @@ NttGeom make_geom(int n) {
     return g;
 }
 
-// Column batch: the passes are integer-pipe bound (ncu: DRAM < 15 % busy), so filling the machine evenly matters more than
-// keeping the intermediates L2-resident: a batch is 16 tiles per SM.  PB_LDE_BATCH overrides for experiments.
+// Column batch: 16 tiles per SM (66 columns at 2^20 on 132 SMs).  On the H100 the passes run at 40-75 % of HBM bandwidth and
+// 3-6 butterflies/clk/SM (scripts/lde_kernels.py); batches of 2-16 columns, alone or round-robin over 2-8 streams so that the
+// K1->K2->K3 intermediates of the batches in flight fit the 50 MB L2, measured no faster at 2022 or 3348 columns
+// (scripts/lde_sweep.py, DESIGN.md §4).  PB_LDE_BATCH / PB_LDE_STREAMS override for experiments.
 size_t lde_column_batch(const pb_ctx* ctx, size_t N, size_t width) {
     const size_t tiles_per_col = std::max<size_t>(1, N >> ntt::LOG_TILE_MAX);
     size_t batch = std::max<size_t>(1, (size_t)ctx->n_sms * 16 / tiles_per_col);

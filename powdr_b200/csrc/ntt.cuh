@@ -12,8 +12,8 @@
 //       K2a inverse, bits [0,n_lo)   transposed tiles [2^n_lo rows x 32 lanes], lane = one contiguous 2^n_lo block
 //       K2b forward, bits [0,n_lo)   per coset, same geometry
 //       K3  forward, bits [n_lo,n)   per coset, strided tiles, then the bit-reversed store
-//     Each column crosses HBM once in (4N bytes) and once out (4N*2^b); the batch is sized to fill the SMs, not to keep the
-//     intermediates in the 50 MB L2 (the passes are integer-pipe bound).
+//     Each pass reads and writes its column batch through HBM (11 words per element at b = 1); the batch is sized to fill the
+//     SMs, not to keep the intermediates in the 50 MB L2 (smaller, L2-sized batches measured no faster, capi.cu).
 //   * inside a pass the butterfly network never crosses lanes: a thread owns 2^q (q<=5) rows of one lane in REGISTERS and
 //     runs q radix-2 stages on them (80 butterflies per 32 loads + 32 stores for q=5); shared memory is touched once per
 //     round, conflict-free (lane = bank, XOR swizzle for the two transposed accesses).

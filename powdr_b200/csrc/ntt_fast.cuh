@@ -34,50 +34,49 @@ __device__ __forceinline__ uint32_t sidx(uint32_t t, uint32_t j) {
 // Q radix-2 stages in registers.  Twiddles are (w, w') pairs for Shoup's constant product (w canonical, w' = floor(w 2^32/p)):
 // IMAD.HI + 2 IMAD = 8 FMA-pipe cycles instead of 10, lazy [0,2p) operands accepted, data stays in Montgomery form.
 // KS = twiddle-index stride of local bit 0.
-template <int Q, bool INV, int KS>
-__device__ __forceinline__ void stages(uint32_t (&x)[1 << Q], const uint2* __restrict__ tw, int u0, uint32_t koff, bool last_inverse,
-                                       uint2 ninv) {
-    if (INV) {
+//
+// Every loop below has a compile-time trip count (the stage index S is a template parameter, stages recurse over it), so x[]
+// stays in registers.  With the stage index a run-time loop variable, the inner trip count 1 << s depends on it and NVVM for
+// sm_90 leaves the Q = 5 stage loops rolled: x[32] then lives in a 128-byte stack frame and every stage round-trips it through
+// local memory.
+template <int Q, int S, bool INV, int KS>
+__device__ __forceinline__ void stage(uint32_t (&x)[1 << Q], const uint2* __restrict__ t) {
 #pragma unroll
-        for (int s = Q - 1; s >= 0; s--) {
-            if (s == 0 && last_inverse) {
+    for (int el = 0; el < (1 << S); el++) {
+        const uint2 w = __ldg(t + (size_t)el * KS);
 #pragma unroll
-                for (int e = 0; e < (1 << Q); e += 2) {
-                    uint32_t a = x[e], b = x[e + 1];
-                    x[e] = bb::mul_shoup(a + b, ninv);
-                    x[e + 1] = bb::mul_shoup(a - b + bb::P, ninv);
-                }
+        for (int eh = 0; eh < (1 << (Q - 1 - S)); eh++) {
+            const int e = (eh << (S + 1)) | el;
+            if constexpr (INV) {
+                uint32_t a = x[e], b = x[e | (1 << S)];
+                x[e] = bb::add(a, b);
+                x[e | (1 << S)] = bb::mul_shoup(a - b + bb::P, w);      // lazy difference in (0, 2p)
             } else {
-                const uint2* t = tw + ((size_t)1 << (u0 + s)) + koff;
-#pragma unroll
-                for (int el = 0; el < (1 << s); el++) {
-                    const uint2 w = __ldg(t + (size_t)el * KS);
-#pragma unroll
-                    for (int eh = 0; eh < (1 << (Q - 1 - s)); eh++) {
-                        const int e = (eh << (s + 1)) | el;
-                        uint32_t a = x[e], b = x[e | (1 << s)];
-                        x[e] = bb::add(a, b);
-                        x[e | (1 << s)] = bb::mul_shoup(a - b + bb::P, w);      // lazy difference in (0, 2p)
-                    }
-                }
+                uint32_t a = x[e], m = bb::mul_shoup(x[e | (1 << S)], w);
+                x[e] = bb::add(a, m);
+                x[e | (1 << S)] = bb::sub(a, m);
             }
         }
-    } else {
+    }
+}
+
+// Inverse: stages Q-1 .. 0 (DIF); forward: stages 0 .. Q-1 (DIT).  LAST_INV: stage 0 is the last of the whole inverse
+// transform, whose twiddle is 1, and folds in the 1/N scale instead.
+template <int Q, bool INV, int KS, bool LAST_INV, int I = 0>
+__device__ __forceinline__ void stages(uint32_t (&x)[1 << Q], const uint2* __restrict__ tw, int u0, uint32_t koff, uint2 ninv) {
+    if constexpr (I < Q) {
+        constexpr int S = INV ? Q - 1 - I : I;
+        if constexpr (INV && LAST_INV && S == 0) {
 #pragma unroll
-        for (int s = 0; s < Q; s++) {
-            const uint2* t = tw + ((size_t)1 << (u0 + s)) + koff;
-#pragma unroll
-            for (int el = 0; el < (1 << s); el++) {
-                const uint2 w = __ldg(t + (size_t)el * KS);
-#pragma unroll
-                for (int eh = 0; eh < (1 << (Q - 1 - s)); eh++) {
-                    const int e = (eh << (s + 1)) | el;
-                    uint32_t a = x[e], m = bb::mul_shoup(x[e | (1 << s)], w);
-                    x[e] = bb::add(a, m);
-                    x[e | (1 << s)] = bb::sub(a, m);
-                }
+            for (int e = 0; e < (1 << Q); e += 2) {
+                uint32_t a = x[e], b = x[e + 1];
+                x[e] = bb::mul_shoup(a + b, ninv);
+                x[e + 1] = bb::mul_shoup(a - b + bb::P, ninv);
             }
+        } else {
+            stage<Q, S, INV, KS>(x, tw + ((size_t)1 << (u0 + S)) + koff);
         }
+        stages<Q, INV, KS, LAST_INV, I + 1>(x, tw, u0, koff, ninv);
     }
 }
 
@@ -101,7 +100,7 @@ __device__ __forceinline__ void round_dev(uint32_t* __restrict__ sm, const uint2
             x[e] = G_IN ? __ldg(gsrc + ((size_t)t << UB) + j) : sm[sidx<RB, LLC, SWZ>(t, j)];
         }
         const uint32_t koff = (LANE_K ? j : 0u) + (tl << UB);
-        stages<Q, INV, KS>(x, tw, UB + B0, koff, INV && UB == 0 && B0 == 0, ninv);
+        stages<Q, INV, KS, INV && UB == 0 && B0 == 0>(x, tw, UB + B0, koff, ninv);
 #pragma unroll
         for (int e = 0; e < (1 << Q); e++) {
             const uint32_t t = tbase + ((uint32_t)e << B0);

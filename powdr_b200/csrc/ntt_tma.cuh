@@ -66,7 +66,7 @@ __device__ __forceinline__ void round_a(uint32_t* blk, uint32_t lane, const uint
     uint32_t x[32];
 #pragma unroll
     for (int e = 0; e < 32; e++) x[e] = blk[32 * e + (lane ^ ((e & 7) << 2))];
-    nttf::stages<5, INV, 32>(x, tw, 5, lane, false, ninv);
+    nttf::stages<5, INV, 32, false>(x, tw, 5, lane, ninv);
 #pragma unroll
     for (int e = 0; e < 32; e++) blk[32 * e + (lane ^ ((e & 7) << 2))] = x[e];
 }
@@ -80,15 +80,18 @@ __device__ __forceinline__ void round_b(uint32_t* blk, uint32_t lane, const uint
         const uint4 v = row[c ^ (lane & 7)];
         x[4 * c] = v.x; x[4 * c + 1] = v.y; x[4 * c + 2] = v.z; x[4 * c + 3] = v.w;
     }
-    nttf::stages<5, INV, 1>(x, tw, 0, 0u, INV, ninv);
+    nttf::stages<5, INV, 1, INV>(x, tw, 0, 0u, ninv);
 #pragma unroll
     for (int c = 0; c < 8; c++) row[c ^ (lane & 7)] = make_uint4(x[4 * c], x[4 * c + 1], x[4 * c + 2], x[4 * c + 3]);
 }
 
 // tm_src / tm_dst: 2-D tensor maps {32 words, rows} with 128 B swizzle and a {32, 256} box over the source / destination buffers.
 // src tile of CTA x = rows [x * 512, (x + 1) * 512); dst rows = ((col * cosets + c) << (n - 5)) + (blk_in_col << 5).
+// The inverse pass is capped at 2 CTAs per SM instead of 3: under the 80-register cap of 3 CTAs, ptxas spills 124 bytes of it
+// (round B's warp-uniform twiddles and the 1/N pair on top of x[32]).  At 2^20 x 2022 on the H100 the 121-register version
+// takes 6.8 ms against 8.7 ms with the spill (DESIGN.md §4).
 template <bool INV>
-__global__ void __launch_bounds__(THREADS, 3) transposed_tma_kernel(const __grid_constant__ CUtensorMap tm_src, const __grid_constant__ CUtensorMap tm_dst, int n,
+__global__ void __launch_bounds__(THREADS, INV ? 2 : 3) transposed_tma_kernel(const __grid_constant__ CUtensorMap tm_src, const __grid_constant__ CUtensorMap tm_dst, int n,
                                                                  int log_blowup, const uint2* __restrict__ tw_all, uint2 ninv) {
     extern __shared__ uint8_t smem_raw[];
     __shared__ __align__(8) uint64_t bar;
