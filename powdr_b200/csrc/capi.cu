@@ -8,6 +8,7 @@
 #include <stdlib.h>
 #include <string.h>
 #include <algorithm>
+#include <memory>
 #include <unordered_map>
 #include <vector>
 
@@ -31,6 +32,11 @@
     do {                                       \
         cudaError_t e__ = (x);                 \
         if (e__ != cudaSuccess) return (int)e__; \
+    } while (0)
+#define RC(x)                          \
+    do {                               \
+        const int r__ = (x);           \
+        if (r__) return r__;           \
     } while (0)
 #define LAUNCHED(ctx) ((ctx)->launches++)
 
@@ -83,10 +89,14 @@ struct TwiddleSet {
     uint2* d_fwd;        // [cosets][2^n]   tw_fwd[c][2^u + k] = S_c^(2^(n-1-u)) * w_{2^(u+1)}^{k},  S_c = shift * w_{N 2^b}^c
 };
 
+// device buffer that grows on demand and frees itself; move-only (noexcept, so that a std::vector of holders can resize)
 template <typename T>
 struct DevBuf {
     T* p = nullptr;
     size_t cap = 0;
+    DevBuf() = default;
+    DevBuf(DevBuf&& o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+    ~DevBuf() { if (p) cudaFree(p); }
     int ensure(size_t n) {
         if (n <= cap) return 0;
         if (p) cudaFree(p);
@@ -97,7 +107,6 @@ struct DevBuf {
         cap = n;
         return 0;
     }
-    void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
 };
 
 __global__ void to_monty_kernel(uint32_t* a, size_t n) {
@@ -113,10 +122,10 @@ __global__ void from_monty_kernel(uint32_t* a, size_t n) {
 
 struct pb_air {
     uint32_t width = 0, n_constraints = 0;
-    uint32_t* d_code = nullptr;
-    air::Span* d_spans = nullptr;
-    uint32_t* d_pool = nullptr;
-    uint32_t* d_alpha_pows = nullptr;   // [C][4]
+    DevBuf<uint32_t> d_code;
+    DevBuf<air::Span> d_spans;
+    DevBuf<uint32_t> d_pool;
+    DevBuf<uint32_t> d_alpha_pows;      // [C][4]
     size_t n_code = 0, n_pool = 0;
     airjit::Kernel jit;                 // NVRTC-compiled straight-line evaluator of this AIR
     bool jit_ok = false;
@@ -124,9 +133,9 @@ struct pb_air {
     bool has_lu = false;
     logup::Program lu;
     logup::Kernels lujit;
-    uint4* d_kc = nullptr;              // [n_ints]   alpha_lu + beta^k (bus+1) + literal arguments
-    uint4* d_bt = nullptr;              // [max_args + 1] beta powers
-    uint4* d_apl = nullptr;             // [n_chunks] alpha^(n_chunks + 2 - c)
+    DevBuf<uint4> d_kc;                 // [n_ints]   alpha_lu + beta^k (bus+1) + literal arguments
+    DevBuf<uint4> d_bt;                 // [max_args + 1] beta powers
+    DevBuf<uint4> d_apl;                // [n_chunks] alpha^(n_chunks + 2 - c)
 };
 
 struct pb_bus {
@@ -155,11 +164,10 @@ struct pb_ctx {
     DevBuf<uint32_t> tmp, tmp2;       // LDE intermediates (L2-sized)
     DevBuf<const uint32_t*> coltab;
     // pb_prove_segment workspace
-    DevBuf<uint32_t> ws_trace, ws_lde, ws_layers, ws_q, ws_qnat, ws_qlde, ws_f0, ws_f1, ws_state, ws_ys;
+    DevBuf<uint32_t> ws_trace, ws_lde, ws_layers, ws_q, ws_qnat, ws_qlde, ws_f0, ws_state, ws_ys;
     DevBuf<uint4> ws_w, ws_part;          // barycentric weights [N], per-CTA partial sums of the openings
     DevBuf<uint2> ws_gp;                  // gamma powers of the reduced opening, canonical (one uint4 per column)
-    DevBuf<const uint32_t*> coltab2;
-    DevBuf<uint32_t> ws_layers_q, ws_layers_open, ws_fri_words, ws_fri_trees, ws_qidx, ws_qout;
+    DevBuf<uint32_t> ws_layers_q, ws_fri_words, ws_fri_trees, ws_qidx, ws_qout;
     DevBuf<uint32_t> ws_shard_send, ws_shard_recv, ws_shard_coef, ws_gather, ws_gather2;   // multi-GPU segment (shard_api.inl)
     DevBuf<uint32_t> ws_qraw;             // running constraint fold between the chunks of a JIT-compiled AIR, [4][rows]
     DevBuf<uint32_t> ws_perm, ws_perm_lde, ws_layers_p, ws_rowsum, ws_scan_tot, ws_lu_raw, ws_lu_s, ws_pow;   // LogUp phase + PoW
@@ -385,24 +393,13 @@ int pb_ctx_destroy(pb_ctx_t* ctx) {
     cudaStreamSynchronize(ctx->stream);
     for (auto& t : ctx->tws) { cudaFree(t.d_inv); cudaFree(t.d_fwd); }
     if (ctx->d_fold_tab) cudaFree(ctx->d_fold_tab);
-    ctx->tmp.release(); ctx->tmp2.release(); ctx->coltab.release();
-    ctx->ws_trace.release(); ctx->ws_lde.release(); ctx->ws_layers.release(); ctx->ws_q.release();
-    ctx->ws_ys.release(); ctx->ws_w.release(); ctx->ws_part.release(); ctx->ws_gp.release(); ctx->coltab2.release();
-    ctx->ws_layers_q.release(); ctx->ws_layers_open.release(); ctx->ws_fri_words.release(); ctx->ws_fri_trees.release();
-    ctx->ws_qidx.release(); ctx->ws_qout.release();
-    ctx->ws_perm.release(); ctx->ws_perm_lde.release(); ctx->ws_layers_p.release(); ctx->ws_rowsum.release(); ctx->ws_scan_tot.release();
-    ctx->ws_lu_raw.release(); ctx->ws_lu_s.release(); ctx->ws_pow.release();
-    ctx->ws_qraw.release(); ctx->ws_shard_send.release(); ctx->ws_shard_recv.release(); ctx->ws_shard_coef.release(); ctx->ws_gather.release(); ctx->ws_gather2.release();
-    ctx->ws_qnat.release(); ctx->ws_qlde.release(); ctx->ws_f0.release(); ctx->ws_f1.release(); ctx->ws_state.release();
-    ctx->ws_fri_ch.release(); ctx->ws_fri_log.release(); ctx->ws_sh_q.release(); ctx->ws_sh_qall.release();
-    ctx->ws_mc_dig.release(); ctx->mc.tree_main.release(); ctx->mc.tree_perm.release(); ctx->mc.tree_q.release();
-    for (auto& b : ctx->mc.ro) b.release();
-    for (auto& w : ctx->mc.chips) { w.lde.release(); w.perm.release(); w.perm_lde.release(); w.qnat.release(); w.qlde.release(); }
     if (ctx->copy_stream) cudaStreamDestroy(ctx->copy_stream);
+    for (int i = 0; i < 8; i++) { if (ctx->lde_streams[i]) cudaStreamDestroy(ctx->lde_streams[i]); if (ctx->lde_join[i]) cudaEventDestroy(ctx->lde_join[i]); }
+    if (ctx->lde_fork) cudaEventDestroy(ctx->lde_fork);
     for (int i = 0; i < 2; i++) { if (ctx->ev_copy[i]) cudaEventDestroy(ctx->ev_copy[i]); if (ctx->ev_free[i]) cudaEventDestroy(ctx->ev_free[i]); }
     for (auto& e : ctx->ev) if (e) cudaEventDestroy(e);
     for (int i = 0; i < pb_ctx::KPROF; i++) { if (ctx->kp_a[i]) cudaEventDestroy(ctx->kp_a[i]); if (ctx->kp_b[i]) cudaEventDestroy(ctx->kp_b[i]); }
-    delete ctx;
+    delete ctx;                                  // the workspaces free themselves
     return 0;
 }
 
@@ -683,21 +680,21 @@ int pb_air_compile(pb_ctx_t* ctx, const uint32_t* bc, size_t n_words, const pb_e
         int prc = pack_program(bc, n_words, cons, n_constraints, width, code, pool, spans);
         if (prc) return prc;
     }
-    pb_air* a = new pb_air();
+    std::unique_ptr<pb_air> a(new pb_air());          // an early return below frees it and its buffers
     a->width = width;
     a->n_constraints = (uint32_t)n_constraints;
     a->n_code = code.size();
     a->n_pool = pool.size();
-    CK(cudaMalloc((void**)&a->d_code, std::max<size_t>(1, code.size()) * 4));
-    CK(cudaMalloc((void**)&a->d_spans, std::max<size_t>(1, spans.size()) * sizeof(air::Span)));
-    CK(cudaMalloc((void**)&a->d_pool, std::max<size_t>(1, pool.size()) * 4));
-    CK(cudaMalloc((void**)&a->d_alpha_pows, std::max<size_t>(1, n_constraints) * 16));
-    CK(cudaMemcpyAsync(a->d_code, code.data(), code.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaMemcpyAsync(a->d_spans, spans.data(), spans.size() * sizeof(air::Span), cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaMemcpyAsync(a->d_pool, pool.data(), pool.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
+    RC(a->d_code.ensure(std::max<size_t>(1, code.size())));
+    RC(a->d_spans.ensure(std::max<size_t>(1, spans.size())));
+    RC(a->d_pool.ensure(std::max<size_t>(1, pool.size())));
+    RC(a->d_alpha_pows.ensure(4 * std::max<size_t>(1, n_constraints)));
+    CK(cudaMemcpyAsync(a->d_code.p, code.data(), code.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(a->d_spans.p, spans.data(), spans.size() * sizeof(air::Span), cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(a->d_pool.p, pool.data(), pool.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     a->jit_ok = n_constraints > 0 && airjit::build(code, spans, pool, &a->jit) == 0;   // straight-line per-AIR kernel (air_jit.cuh)
-    *out = a;
+    *out = a.release();
     return 0;
 }
 
@@ -707,8 +704,6 @@ int pb_air_free(pb_air_t* a) {
     if (!a) return 0;
     if (a->jit_ok) airjit::destroy(a->jit);
     if (a->has_lu) logup::destroy(a->lujit);
-    cudaFree(a->d_kc); cudaFree(a->d_bt); cudaFree(a->d_apl);
-    cudaFree(a->d_code); cudaFree(a->d_spans); cudaFree(a->d_pool); cudaFree(a->d_alpha_pows);
     delete a;
     return 0;
 }
@@ -723,8 +718,16 @@ static int upload_alpha_pows(pb_ctx* ctx, const pb_air* a, bb::E4 alpha, size_t 
         memcpy(&ap[4 * k], cur.c, 16);
         cur = bb::e4_mul(cur, alpha);
     }
-    CK(cudaMemcpyAsync(a->d_alpha_pows, ap.data(), 16 * C, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(a->d_alpha_pows.p, ap.data(), 16 * C, cudaMemcpyHostToDevice, ctx->stream));
     return 0;
+}
+
+// Z_H(x) = x^N - 1 on the two cosets s*H and s*w_2N*H of the LDE domain (log_blowup 1) is s^N - 1 and -s^N - 1:
+// sn = s^N, zinv0 / zinv1 = their inverses (Montgomery)
+static void zh_inverses(size_t log_n, uint32_t shift_m, uint32_t* sn, uint32_t* zinv0, uint32_t* zinv1) {
+    *sn = bb::pow(shift_m, (uint64_t)1 << log_n);
+    *zinv0 = bb::inv(bb::sub(*sn, bb::R1));
+    *zinv1 = bb::inv(bb::sub(bb::neg(*sn), bb::R1));
 }
 
 int pb_quotient(pb_ctx_t* ctx, const pb_air_t* a, const uint32_t* d_lde, size_t log_n, uint32_t log_blowup, uint32_t shift,
@@ -733,17 +736,17 @@ int pb_quotient(pb_ctx_t* ctx, const pb_air_t* a, const uint32_t* d_lde, size_t 
     if (log_blowup != 1 || log_n < 1 || log_n > 26) return PB_ERR_UNSUPPORTED;
     int rc = upload_alpha_pows(ctx, a, h_e4_from_canon(alpha));
     if (rc) return rc;
-    const uint32_t sn = bb::pow(h_to_m(shift), (uint64_t)1 << log_n);
-    const uint32_t zinv0 = bb::inv(bb::sub(sn, bb::R1)), zinv1 = bb::inv(bb::sub(bb::neg(sn), bb::R1));
+    uint32_t sn, zinv0, zinv1;
+    zh_inverses(log_n, h_to_m(shift), &sn, &zinv0, &zinv1);
     const size_t m = (size_t)2 << log_n;
     if (a->jit_ok) {
         if (a->jit.fns.size() > 1) { rc = ctx->ws_qraw.ensure(4 * m); if (rc) return rc; }
-        rc = airjit::launch(a->jit, ctx->stream, d_lde, m, (int)log_n, a->d_alpha_pows, zinv0, zinv1, d_q, 1, ctx->ws_qraw.p);
+        rc = airjit::launch(a->jit, ctx->stream, d_lde, m, (int)log_n, a->d_alpha_pows.p, zinv0, zinv1, d_q, 1, ctx->ws_qraw.p);
         LAUNCHED(ctx);
         return rc;
     }
     air::quotient_kernel<<<(unsigned)((m + air::THREADS - 1) / air::THREADS), air::THREADS, 0, ctx->stream>>>(
-        a->d_code, a->d_spans, a->n_constraints, a->d_pool, d_lde, (int)log_n, a->d_alpha_pows, zinv0, zinv1, d_q, 1);
+        a->d_code.p, a->d_spans.p, a->n_constraints, a->d_pool.p, d_lde, (int)log_n, a->d_alpha_pows.p, zinv0, zinv1, d_q, 1);
     LAUNCHED(ctx);
     CK(cudaGetLastError());
     return 0;
@@ -761,12 +764,12 @@ static int constraint_fold_m(pb_ctx* ctx, const pb_air* a, const uint32_t* d_mat
     if (a->n_constraints == 0) { CK(cudaMemsetAsync(d_out, 0, 16 * height, ctx->stream)); return 0; }
     if (a->jit_ok) {
         if (a->jit.fns.size() > 1) { rc = ctx->ws_qraw.ensure(4 * height); if (rc) return rc; }
-        rc = airjit::launch(a->jit, ctx->stream, d_mat, height, 0, a->d_alpha_pows, 0u, 0u, d_out, 0, ctx->ws_qraw.p);
+        rc = airjit::launch(a->jit, ctx->stream, d_mat, height, 0, a->d_alpha_pows.p, 0u, 0u, d_out, 0, ctx->ws_qraw.p);
         LAUNCHED(ctx);
         return rc;
     }
     air::constraint_fold_kernel<<<(unsigned)((height + air::THREADS - 1) / air::THREADS), air::THREADS, 0, ctx->stream>>>(
-        a->d_code, a->d_spans, a->n_constraints, a->d_pool, d_mat, height, a->d_alpha_pows, d_out);
+        a->d_code.p, a->d_spans.p, a->n_constraints, a->d_pool.p, d_mat, height, a->d_alpha_pows.p, d_out);
     LAUNCHED(ctx);
     CK(cudaGetLastError());
     return 0;
@@ -1019,12 +1022,6 @@ static int deep_quotient_groups_m(pb_ctx* ctx, const std::vector<const uint32_t*
     CK(cudaGetLastError());
     return 0;
 }
-static int deep_quotient_m(pb_ctx* ctx, const std::vector<const uint32_t*>& cols, size_t log_m, uint32_t shift_m, bb::E4 zeta_m,
-                           bb::E4 gamma_m, const uint32_t* ys_m, uint32_t* d_out, size_t row0 = 0, size_t n_rows = 0) {
-    return deep_quotient_groups_m(ctx, cols, std::vector<uint32_t>(cols.size(), 0u), std::vector<bb::E4>{zeta_m}, log_m, shift_m, gamma_m, ys_m, d_out,
-                                  row0, n_rows);
-}
-
 int pb_eval_at_point(pb_ctx_t* ctx, const uint32_t* d_mat, size_t log_n, size_t width, uint32_t shift, const uint32_t zeta[4], uint32_t* d_ys) {
     if (!ctx || !d_mat || !zeta || !d_ys) return PB_ERR_INVALID_ARG;
     if (log_n < 1 || log_n > 27 || shift == 0 || shift >= bb::P) return PB_ERR_UNSUPPORTED;
@@ -1041,7 +1038,8 @@ int pb_deep_quotient(pb_ctx_t* ctx, const uint32_t* const* d_mats, const size_t*
     std::vector<uint32_t> ys(4 * cols.size());
     CK(cudaMemcpyAsync(ys.data(), d_ys, 16 * cols.size(), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
-    return deep_quotient_m(ctx, cols, log_m, h_to_m(shift), h_e4_from_canon(zeta), h_e4_from_canon(gamma), ys.data(), d_out);
+    return deep_quotient_groups_m(ctx, cols, std::vector<uint32_t>(cols.size(), 0u), {h_e4_from_canon(zeta)}, log_m, h_to_m(shift),
+                                  h_e4_from_canon(gamma), ys.data(), d_out);
 }
 
 #include "segment.inl"

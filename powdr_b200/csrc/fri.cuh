@@ -41,44 +41,13 @@ __global__ void __launch_bounds__(256) add_words_kernel(uint32_t* __restrict__ f
     if (i < n) f[i] = bb::add(f[i], g[i]);
 }
 
-// FRI input codeword from the two committed quotient-chunk LDEs (8 base columns, column-major, height m):
-// f[r] = Q0[r] + gamma * Q1[r]
-__global__ void __launch_bounds__(256) combine_chunks_kernel(const uint32_t* __restrict__ qlde, size_t m, bb::E4 gamma, uint4* __restrict__ f) {
-    size_t r = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (r >= m) return;
-    bb::E4 a, b;
-#pragma unroll
-    for (int l = 0; l < 4; l++) { a.c[l] = __ldg(qlde + (size_t)l * m + r); b.c[l] = __ldg(qlde + (size_t)(4 + l) * m + r); }
-    bb::E4 v = bb::e4_add(a, bb::e4_mul(gamma, b));
-    f[r] = make_uint4(v.c[0], v.c[1], v.c[2], v.c[3]);
-}
-
 }  // namespace fri
 
 // ---------------- query phase: gather the openings a verifier needs for each sampled index (SURVEY.md §8f-4) ----------------
-// One CTA per query.  Output (canonical words) per query:
-//   [ r | trace row (W) | trace path (log_m x 8) | perm row (Wp) | perm path (log_m x 8)  (when Wp > 0) | quotient row (8) | quotient path (log_m x 8) |
-//     per FRI layer i: pair row (8), path ((log_m-1-i) x 8) ]
+// One CTA per query and one launch per piece of the layout (include/powdr_b200.h): the index; per commitment the row of each of its
+// matrices, then the Merkle path; per FRI layer i the opened pair and its path ((log_max-1-i) x 8).  All words canonical.
 // Merkle trees are node-major with level k at node offset 2^(h+1) - 2^(h-k+1); the sibling of leaf idx at level k is (idx>>k)^1.
 namespace fri {
-
-struct QueryDesc {
-    const uint32_t* lde;        // trace LDE, column-major [W][M]
-    const uint32_t* qlde;       // quotient chunk LDEs, column-major [8][M]
-    const uint32_t* tree_t;     // digest layers of the trace commitment
-    const uint32_t* tree_q;     // digest layers of the quotient commitment
-    const uint32_t* plde;       // LogUp permutation-trace LDE, column-major [perm_width][M] (unused when perm_width = 0)
-    const uint32_t* tree_p;     // digest layers of the permutation-trace commitment
-    uint32_t perm_width;
-    const uint32_t* fri_words;  // all FRI codewords back to back (layer i at word_off[i])
-    const uint32_t* fri_trees;  // all FRI layer trees back to back (layer i at tree_off[i], in words)
-    size_t m;
-    uint32_t width;
-    int log_m;
-    int n_layers;
-    size_t word_off[32];
-    size_t tree_off[32];
-};
 
 __device__ __forceinline__ void copy_path(const uint32_t* tree, int log_h, size_t idx, uint32_t* out) {
     for (int k = 0; k < log_h; k++) {
@@ -88,41 +57,6 @@ __device__ __forceinline__ void copy_path(const uint32_t* tree, int log_h, size_
     }
 }
 
-__global__ void __launch_bounds__(256) gather_queries_kernel(QueryDesc d, const uint32_t* __restrict__ indices, uint32_t* __restrict__ out,
-                                                             size_t words_per_query) {
-    const size_t r = indices[blockIdx.x];
-    uint32_t* o = out + (size_t)blockIdx.x * words_per_query;
-    if (threadIdx.x == 0) o[0] = (uint32_t)r;
-    o += 1;
-    for (uint32_t c = threadIdx.x; c < d.width; c += blockDim.x) o[c] = bb::from_monty(d.lde[(size_t)c * d.m + r]);
-    o += d.width;
-    copy_path(d.tree_t, d.log_m, r, o);
-    o += 8 * d.log_m;
-    if (d.perm_width) {
-        for (uint32_t c = threadIdx.x; c < d.perm_width; c += blockDim.x) o[c] = bb::from_monty(d.plde[(size_t)c * d.m + r]);
-        o += d.perm_width;
-        copy_path(d.tree_p, d.log_m, r, o);
-        o += 8 * d.log_m;
-    }
-    for (uint32_t c = threadIdx.x; c < 8; c += blockDim.x) o[c] = bb::from_monty(d.qlde[(size_t)c * d.m + r]);
-    o += 8;
-    copy_path(d.tree_q, d.log_m, r, o);
-    o += 8 * d.log_m;
-    for (int i = 0; i < d.n_layers; i++) {
-        const int log_h = d.log_m - 1 - i;
-        const size_t j = r >> (i + 1);
-        const uint32_t* row = d.fri_words + d.word_off[i] + 8 * j;
-        for (uint32_t e = threadIdx.x; e < 8; e += blockDim.x) o[e] = bb::from_monty(row[e]);
-        o += 8;
-        copy_path(d.fri_trees + d.tree_off[i], log_h, j, o);
-        o += 8 * log_h;
-    }
-}
-
-}  // namespace fri
-
-// ---------------- query gathering for the multi-chip prover: generic pieces, one launch per (commitment, matrix) / tree ----------------
-namespace fri {
 // out[q * wpq + off + c] = canonical(mat[c * m + (idx[q] >> shift)])
 __global__ void gather_rows_kernel(const uint32_t* __restrict__ mat, size_t m, uint32_t width, int shift, const uint32_t* __restrict__ idx, uint32_t* __restrict__ out,
                                    size_t wpq, size_t off) {
