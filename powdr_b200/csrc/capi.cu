@@ -8,8 +8,10 @@
 #include <stdlib.h>
 #include <string.h>
 #include <algorithm>
+#include <array>
 #include <memory>
 #include <unordered_map>
+#include <utility>
 #include <vector>
 
 #include "../../include/pb_poseidon2_constants.h"
@@ -352,6 +354,102 @@ int read_root(pb_ctx* ctx, const uint32_t* d_layers, size_t log_h, uint32_t root
     return 0;
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// The two halves of the LDE (shared by pb_lde_batch and pb_lde_shard), with the pass plan of each log_n fixed at compile time
+
+// Column batch: 16 tiles of 2^LDE_BATCH_LOG_TILE elements per SM (66 columns at 2^20 on 132 SMs).  On the H100 the passes run
+// at 40-75 % of HBM bandwidth and 3-6 butterflies/clk/SM (scripts/lde_kernels.py); batches of 2-16 columns, alone or round-robin
+// over 2-8 streams so that the K1->K2->K3 intermediates of the batches in flight fit the 50 MB L2, measured no faster at 2022 or
+// 3348 columns (scripts/lde_sweep.py, DESIGN.md §4).  PB_LDE_BATCH / PB_LDE_STREAMS override for experiments.
+constexpr int LDE_BATCH_LOG_TILE = 15;
+size_t lde_column_batch(const pb_ctx* ctx, size_t N, size_t width) {
+    const size_t tiles_per_col = std::max<size_t>(1, N >> LDE_BATCH_LOG_TILE);
+    size_t batch = std::max<size_t>(1, (size_t)ctx->n_sms * 16 / tiles_per_col);
+    if (const char* e = getenv("PB_LDE_BATCH")) batch = std::max<size_t>(1, (size_t)atol(e));
+    batch = std::min<size_t>(std::min<size_t>(batch, width), 32768);
+    return (width + (width + batch - 1) / batch - 1) / ((width + batch - 1) / batch);     // equal-sized batches (no runt batch)
+}
+
+// K1 + K2a: nb natural-order columns (stride N) -> coefficients in bit-reversed slots, scaled by 1/N, in coef (stride N)
+template <int LOG_N>
+void inverse_passes(pb_ctx* ctx, const TwiddleSet* tw, const uint32_t* src, unsigned nb, uint32_t* coef) {
+    constexpr int LO = nttf::n_lo_of(LOG_N), HI = LOG_N - LO;
+    constexpr size_t N = (size_t)1 << LOG_N;
+    if constexpr (HI > 0) {
+        const dim3 g1(1u << (LO - nttf::log_lc_of(HI)), nb);
+        nttf::strided_kernel<HI, LO, true><<<g1, nttf::THREADS, nttf::tile_bytes(HI), ctx->stream>>>(src, N, coef, N, 0, tw->d_inv);
+        LAUNCHED(ctx);
+        src = coef;
+    }
+    const size_t total_blocks = (size_t)nb << HI;
+    // n_lo == 10: the TMA-staged kernel (ntt_tma.cuh) where its preconditions hold
+    if (!ntttma::launch_transposed(true, LOG_N, LO, ctx->stream, src, coef, 0, total_blocks, nb * N, nb * N, tw->d_inv, tw->ninv)) {
+        const dim3 g2((unsigned)((total_blocks + ((size_t)1 << nttf::log_lc_of(LO)) - 1) >> nttf::log_lc_of(LO)));
+        nttf::transposed_kernel<LO, true><<<g2, nttf::THREADS, nttf::tile_bytes(LO), ctx->stream>>>(src, N, coef, LOG_N, 0, total_blocks,
+                                                                                                    tw->d_inv, tw->ninv);
+    }
+    LAUNCHED(ctx);
+}
+
+// K2b + K3: coefficients (bit-reversed slots, stride N) -> 2^log_blowup coset evaluations per column, bit-reversed rows,
+// out[col * out_stride + bitrev_b(c) * N + bitrev_n(k)];  scratch holds [nb][cosets][N]
+template <int LOG_N>
+void forward_passes(pb_ctx* ctx, const TwiddleSet* tw, int log_blowup, const uint32_t* coef, unsigned nb, uint32_t* scratch, uint32_t* out,
+                    size_t out_stride) {
+    constexpr int LO = nttf::n_lo_of(LOG_N), HI = LOG_N - LO;
+    constexpr size_t N = (size_t)1 << LOG_N;
+    const unsigned cosets = 1u << log_blowup;
+    const size_t total_blocks = (size_t)nb << HI;
+    if (!ntttma::launch_transposed(false, LOG_N, LO, ctx->stream, coef, scratch, log_blowup, total_blocks, nb * N, nb * N * cosets, tw->d_fwd,
+                                   make_uint2(0u, 0u))) {
+        const dim3 g2((unsigned)((total_blocks + ((size_t)1 << nttf::log_lc_of(LO)) - 1) >> nttf::log_lc_of(LO)), 1, cosets);
+        nttf::transposed_kernel<LO, false><<<g2, nttf::THREADS, nttf::tile_bytes(LO), ctx->stream>>>(coef, N, scratch, LOG_N, log_blowup,
+                                                                                                     total_blocks, tw->d_fwd, make_uint2(0u, 0u));
+    }
+    LAUNCHED(ctx);
+    if constexpr (HI > 0) {
+        const dim3 g3(1u << (LO - nttf::log_lc_of(HI)), nb, cosets);
+        nttf::strided_kernel<HI, LO, false><<<g3, nttf::THREADS, nttf::tile_bytes(HI), ctx->stream>>>(scratch, 0, out, out_stride, log_blowup,
+                                                                                                      tw->d_fwd);
+    } else {
+        const size_t tot = ((size_t)nb * cosets) << LOG_N;
+        ntt::bitrev_store_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, ctx->stream>>>(scratch, out, out_stride, LOG_N, log_blowup, nb);
+    }
+    LAUNCHED(ctx);
+}
+
+// dynamic shared memory opt-in of the passes' kernels on the current device
+template <int LOG_N>
+int opt_in_passes() {
+    constexpr int LO = nttf::n_lo_of(LOG_N), HI = LOG_N - LO, SMEM = 4 << nttf::LOG_TILE;
+    CK(cudaFuncSetAttribute(nttf::transposed_kernel<LO, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
+    CK(cudaFuncSetAttribute(nttf::transposed_kernel<LO, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
+    if constexpr (HI > 0) {
+        CK(cudaFuncSetAttribute(nttf::strided_kernel<HI, LO, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
+        CK(cudaFuncSetAttribute(nttf::strided_kernel<HI, LO, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
+    }
+    return 0;
+}
+
+struct NttPlan {
+    void (*inverse)(pb_ctx*, const TwiddleSet*, const uint32_t*, unsigned, uint32_t*);
+    void (*forward)(pb_ctx*, const TwiddleSet*, int, const uint32_t*, unsigned, uint32_t*, uint32_t*, size_t);
+    int (*opt_in)();
+};
+template <size_t... I>
+constexpr std::array<NttPlan, sizeof...(I)> make_ntt_plans(std::index_sequence<I...>) {
+    return {{{inverse_passes<(int)I + 1>, forward_passes<(int)I + 1>, opt_in_passes<(int)I + 1>}...}};
+}
+constexpr auto NTT_PLANS = make_ntt_plans(std::make_index_sequence<24>());     // NTT_PLANS[log_n - 1], 1 <= log_n <= 24
+
+void ntt_inverse_cols(pb_ctx* ctx, int log_n, const TwiddleSet* tw, const uint32_t* src, unsigned nb, uint32_t* coef) {
+    NTT_PLANS[log_n - 1].inverse(ctx, tw, src, nb, coef);
+}
+void ntt_forward_cols(pb_ctx* ctx, int log_n, const TwiddleSet* tw, int log_blowup, const uint32_t* coef, unsigned nb, uint32_t* scratch,
+                      uint32_t* out, size_t out_stride) {
+    NTT_PLANS[log_n - 1].forward(ctx, tw, log_blowup, coef, nb, scratch, out, out_stride);
+}
+
 }  // namespace
 
 // =====================================================================================================================
@@ -375,10 +473,10 @@ int pb_ctx_create(pb_ctx_t** out, int device, void* cuda_stream) {
             CK(cudaEventCreateWithFlags(&ctx->ev_free[i], cudaEventDisableTiming));
         }
         for (int i = 0; i < pb_ctx::KPROF; i++) { CK(cudaEventCreate(&ctx->kp_a[i])); CK(cudaEventCreate(&ctx->kp_b[i])); }
-        CK(cudaFuncSetAttribute(ntt::strided_pass_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 << ntt::LOG_TILE_MAX));
-        CK(cudaFuncSetAttribute(ntt::strided_pass_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 << ntt::LOG_TILE_MAX));
-        CK(cudaFuncSetAttribute(ntt::transposed_pass_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 << ntt::LOG_TILE_MAX));
-        CK(cudaFuncSetAttribute(ntt::transposed_pass_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 << ntt::LOG_TILE_MAX));
+        // the runtime applies a kernel's shared memory opt-in to the current device only: every context does its own
+        for (const NttPlan& p : NTT_PLANS) RC(p.opt_in());
+        CK(cudaFuncSetAttribute(ntttma::transposed_tma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, ntttma::SMEM_BYTES));
+        CK(cudaFuncSetAttribute(ntttma::transposed_tma_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, ntttma::SMEM_BYTES));
         return upload_p2(ctx, PB_P2_RC_EXT, PB_P2_RC_INT, PB_P2_DIAG_M1);
     };
     const int rc = init();
@@ -463,106 +561,6 @@ int pb_from_monty(pb_ctx_t* ctx, uint32_t* d, size_t n) {
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// ---------------------------------------------------------------------------------------------------------------------
-// NTT pass geometry and the two halves of the LDE (shared by pb_lde_batch and pb_lde_shard)
-namespace {
-
-struct NttGeom {
-    int n, n_lo, n_hi, log_lc_hi, log_lc_lo;
-    bool fast;                          // compile-time specialised passes (ntt_fast.cuh) cover this geometry
-    size_t smem_hi, smem_lo;
-    ntt::Rounds r_inv_hi, r_fwd_hi, r_inv_lo, r_fwd_lo;
-};
-
-NttGeom make_geom(int n) {
-    NttGeom g{};
-    g.n = n;
-    g.n_lo = n <= 10 ? n : (n + 1) / 2;
-    g.n_hi = n - g.n_lo;
-    g.fast = getenv("PB_LDE_GENERIC") == nullptr && nttf::supported(g.n_hi, g.n_lo);
-    // K1/K3 tile: 2^n_hi rows x 2^log_lc_hi lanes;  K2 tile: 2^n_lo rows x 2^log_lc_lo blocks
-    g.log_lc_hi = g.fast ? nttf::log_lc_of(g.n_hi) : std::min(5, ntt::LOG_TILE_MAX - g.n_hi);
-    g.log_lc_lo = g.fast ? nttf::log_lc_of(g.n_lo) : std::min(5, ntt::LOG_TILE_MAX - g.n_lo);
-    g.smem_hi = (size_t)4 << (g.n_hi + g.log_lc_hi);
-    g.smem_lo = (size_t)4 << (g.n_lo + g.log_lc_lo);
-    auto make_rounds = [](int bits, bool descending) {
-        ntt::Rounds r{};
-        const int nr = (bits + 4) / 5;
-        r.n = nr;
-        int q[ntt::MAX_ROUNDS], b0[ntt::MAX_ROUNDS], acc = 0;
-        for (int i = 0; i < nr; i++) { q[i] = bits / nr + (i < bits % nr ? 1 : 0); b0[i] = acc; acc += q[i]; }
-        for (int i = 0; i < nr; i++) { const int k = descending ? nr - 1 - i : i; r.q[i] = q[k]; r.b0[i] = b0[k]; }
-        return r;
-    };
-    g.r_inv_hi = make_rounds(g.n_hi, true); g.r_fwd_hi = make_rounds(g.n_hi, false);
-    g.r_inv_lo = make_rounds(g.n_lo, true); g.r_fwd_lo = make_rounds(g.n_lo, false);
-    return g;
-}
-
-// Column batch: 16 tiles per SM (66 columns at 2^20 on 132 SMs).  On the H100 the passes run at 40-75 % of HBM bandwidth and
-// 3-6 butterflies/clk/SM (scripts/lde_kernels.py); batches of 2-16 columns, alone or round-robin over 2-8 streams so that the
-// K1->K2->K3 intermediates of the batches in flight fit the 50 MB L2, measured no faster at 2022 or 3348 columns
-// (scripts/lde_sweep.py, DESIGN.md §4).  PB_LDE_BATCH / PB_LDE_STREAMS override for experiments.
-size_t lde_column_batch(const pb_ctx* ctx, size_t N, size_t width) {
-    const size_t tiles_per_col = std::max<size_t>(1, N >> ntt::LOG_TILE_MAX);
-    size_t batch = std::max<size_t>(1, (size_t)ctx->n_sms * 16 / tiles_per_col);
-    if (const char* e = getenv("PB_LDE_BATCH")) batch = std::max<size_t>(1, (size_t)atol(e));
-    batch = std::min<size_t>(std::min<size_t>(batch, width), 32768);
-    return (width + (width + batch - 1) / batch - 1) / ((width + batch - 1) / batch);     // equal-sized batches (no runt batch)
-}
-
-// K1 + K2a: nb natural-order columns (stride N) -> coefficients in bit-reversed slots, scaled by 1/N, in coef (stride N)
-void ntt_inverse_cols(pb_ctx* ctx, const NttGeom& g, const TwiddleSet* tw, const uint32_t* src, unsigned nb, uint32_t* coef) {
-    const size_t N = (size_t)1 << g.n;
-    if (g.n_hi > 0) {
-        dim3 g1((unsigned)(1u << (g.n_lo - g.log_lc_hi)), nb);
-        if (!g.fast || !nttf::launch_strided(true, g.n_hi, g.n_lo, g1, ctx->stream, src, N, coef, N, 0, tw->d_inv))
-            ntt::strided_pass_kernel<true><<<g1, ntt::THREADS, g.smem_hi, ctx->stream>>>(src, N, coef, N, g.n, g.n_lo, g.log_lc_hi, 0,
-                                                                                         tw->d_inv, g.r_inv_hi);
-        LAUNCHED(ctx);
-        src = coef;
-    }
-    const size_t total_blocks = (size_t)nb << g.n_hi;
-    const unsigned gx = (unsigned)((total_blocks + ((size_t)1 << g.log_lc_lo) - 1) >> g.log_lc_lo);
-    // n_lo == 10: the TMA-staged kernel (ntt_tma.cuh); otherwise the LDG/STS-staged specialisations, then the generic pass
-    if (g.fast && ntttma::launch_transposed(true, g.n, g.n_lo, ctx->stream, src, coef, 0, total_blocks, (size_t)nb * N, (size_t)nb * N, tw->d_inv, tw->ninv)) {
-    } else if (!g.fast || !nttf::launch_transposed(true, g.n, g.n_lo, dim3(gx), ctx->stream, src, N, coef, 0, total_blocks, tw->d_inv, tw->ninv))
-        ntt::transposed_pass_kernel<true><<<dim3(gx), ntt::THREADS, g.smem_lo, ctx->stream>>>(src, N, coef, g.n, g.n_lo, g.log_lc_lo, 0,
-                                                                                             total_blocks, tw->d_inv, tw->ninv, g.r_inv_lo);
-    LAUNCHED(ctx);
-}
-
-// K2b + K3: coefficients (bit-reversed slots, stride N) -> 2^log_blowup coset evaluations per column, bit-reversed rows,
-// out[col * out_stride + bitrev_b(c) * N + bitrev_n(k)];  scratch holds [nb][cosets][N]
-void ntt_forward_cols(pb_ctx* ctx, const NttGeom& g, const TwiddleSet* tw, int log_blowup, const uint32_t* coef, unsigned nb,
-                      uint32_t* scratch, uint32_t* out, size_t out_stride) {
-    const size_t N = (size_t)1 << g.n;
-    const int cosets = 1 << log_blowup;
-    const size_t total_blocks = (size_t)nb << g.n_hi;
-    const unsigned gx = (unsigned)((total_blocks + ((size_t)1 << g.log_lc_lo) - 1) >> g.log_lc_lo);
-    if (g.fast && ntttma::launch_transposed(false, g.n, g.n_lo, ctx->stream, coef, scratch, log_blowup, total_blocks, (size_t)nb * N,
-                                            (size_t)nb * N * cosets, tw->d_fwd, make_uint2(0u, 0u))) {
-    } else if (!g.fast || !nttf::launch_transposed(false, g.n, g.n_lo, dim3(gx, 1, (unsigned)cosets), ctx->stream, coef, N, scratch, log_blowup,
-                                            total_blocks, tw->d_fwd, make_uint2(0u, 0u)))
-        ntt::transposed_pass_kernel<false><<<dim3(gx, 1, (unsigned)cosets), ntt::THREADS, g.smem_lo, ctx->stream>>>(
-            coef, N, scratch, g.n, g.n_lo, g.log_lc_lo, log_blowup, total_blocks, tw->d_fwd, make_uint2(0u, 0u), g.r_fwd_lo);
-    LAUNCHED(ctx);
-    if (g.n_hi > 0) {
-        dim3 g3((unsigned)(1u << (g.n_lo - g.log_lc_hi)), nb, (unsigned)cosets);
-        if (!g.fast || !nttf::launch_strided(false, g.n_hi, g.n_lo, g3, ctx->stream, scratch, 0, out, out_stride, log_blowup, tw->d_fwd))
-            ntt::strided_pass_kernel<false><<<g3, ntt::THREADS, g.smem_hi, ctx->stream>>>(scratch, 0, out, out_stride, g.n, g.n_lo, g.log_lc_hi,
-                                                                                          log_blowup, tw->d_fwd, g.r_fwd_hi);
-        LAUNCHED(ctx);
-    } else {
-        const size_t tot = ((size_t)nb * cosets) << g.n;
-        ntt::bitrev_store_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, ctx->stream>>>(scratch, out, out_stride, g.n, log_blowup, nb);
-        LAUNCHED(ctx);
-    }
-}
-
-}  // namespace
-
-
 int pb_lde_batch(pb_ctx_t* ctx, const uint32_t* d_trace, size_t log_n, size_t width, uint32_t log_blowup, uint32_t shift,
                  uint32_t* d_lde) {
     if (!ctx || !d_trace || !d_lde) return PB_ERR_INVALID_ARG;
@@ -574,7 +572,6 @@ int pb_lde_batch(pb_ctx_t* ctx, const uint32_t* d_trace, size_t log_n, size_t wi
     const TwiddleSet* tw;
     int rc = get_twiddles(ctx, n, (int)log_blowup, shift, &tw);
     if (rc) return rc;
-    const NttGeom g = make_geom(n);
     const size_t batch = lde_column_batch(ctx, N, width);
     // PB_LDE_STREAMS > 1 (experiment): small column batches round-robin over several streams, so the four passes of different
     // batches overlap and the intermediates of the batches in flight can stay in L2
@@ -600,8 +597,8 @@ int pb_lde_batch(pb_ctx_t* ctx, const uint32_t* d_trace, size_t log_n, size_t wi
         if (n_streams > 1) ctx->stream = ctx->lde_streams[sidx];
         uint32_t* t1 = ctx->tmp.p + sidx * batch * N;
         uint32_t* t2 = ctx->tmp2.p + sidx * batch * N * cosets;
-        ntt_inverse_cols(ctx, g, tw, d_trace + c0 * N, nb, t1);
-        ntt_forward_cols(ctx, g, tw, (int)log_blowup, t1, nb, t2, d_lde + c0 * N * cosets, N * cosets);
+        ntt_inverse_cols(ctx, n, tw, d_trace + c0 * N, nb, t1);
+        ntt_forward_cols(ctx, n, tw, (int)log_blowup, t1, nb, t2, d_lde + c0 * N * cosets, N * cosets);
     }
     ctx->stream = main_stream;
     if (n_streams > 1)

@@ -1,8 +1,8 @@
-// Compile-time specialised LDE passes (same algorithm and tile geometry as ntt.cuh; see the header there).
-// The generic kernels in ntt.cuh spend more than half of their instructions on run-time shifts/masks for tile geometry and
-// round structure (ncu r01: 20-30 instructions per butterfly, ALU pipe 55 % busy with address math).  Here the row-bit
-// count RB, the low split NLO, the round plan (Q, B0) and the lane count are template parameters, so shared/global
-// addressing folds into immediates and each kernel carries only its own two or three register rounds.
+// The LDE passes K1, K2a, K2b, K3 (algorithm: see the header of ntt.cuh), one specialisation per pass geometry.
+// The row-bit count RB, the low split NLO, the round plan (Q, B0) and the lane count are template parameters, so shared/global
+// addressing folds into immediates and each kernel carries only its own two or three register rounds.  Kernels that read
+// their geometry at run time spent more than half of their instructions on shifts/masks for it (ncu r01: 20-30 instructions
+// per butterfly, ALU pipe 55 % busy with address math).
 #pragma once
 #include "bb31.cuh"
 #include "ntt.cuh"
@@ -185,60 +185,10 @@ __global__ void __launch_bounds__(THREADS) transposed_kernel(const uint32_t* __r
     }
 }
 
-}  // namespace nttf
-
-// ---------------- host-side dispatch: returns false when no specialisation covers (n_hi, n_lo) ----------------
-namespace nttf {
-
-template <auto Kernel>
-inline void ensure_smem() {
-    static bool done = false;
-    if (!done) {
-        cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 << LOG_TILE);
-        done = true;
-    }
-}
-
-inline bool launch_strided(bool inv, int n_hi, int n_lo, dim3 grid, cudaStream_t st, const uint32_t* src, size_t src_col_stride,
-                           uint32_t* dst, size_t dst_col_stride, int log_blowup, const uint2* tw) {
-#define PB_CASE(RB, NLO)                                                                                                        \
-    if (n_hi == RB && n_lo == NLO) {                                                                                            \
-        const size_t smem = (size_t)4 << (RB + log_lc_of(RB));                                                                  \
-        if (inv) {                                                                                                              \
-            ensure_smem<strided_kernel<RB, NLO, true>>();                                                                       \
-            strided_kernel<RB, NLO, true><<<grid, THREADS, smem, st>>>(src, src_col_stride, dst, dst_col_stride, log_blowup, tw); \
-        } else {                                                                                                                \
-            ensure_smem<strided_kernel<RB, NLO, false>>();                                                                      \
-            strided_kernel<RB, NLO, false><<<grid, THREADS, smem, st>>>(src, src_col_stride, dst, dst_col_stride, log_blowup, tw); \
-        }                                                                                                                       \
-        return true;                                                                                                            \
-    }
-    PB_CASE(8, 8) PB_CASE(8, 9) PB_CASE(9, 9) PB_CASE(9, 10) PB_CASE(10, 10) PB_CASE(10, 11) PB_CASE(11, 11) PB_CASE(11, 12) PB_CASE(12, 12)
-#undef PB_CASE
-    return false;
-}
-
-inline bool launch_transposed(bool inv, int n, int n_lo, dim3 grid, cudaStream_t st, const uint32_t* src, size_t src_col_stride,
-                              uint32_t* dst, int log_blowup, size_t total_blocks, const uint2* tw, uint2 ninv) {
-#define PB_CASE(RB)                                                                                                               \
-    if (n_lo == RB) {                                                                                                             \
-        const size_t smem = (size_t)4 << (RB + log_lc_of(RB));                                                                    \
-        if (inv) {                                                                                                                \
-            ensure_smem<transposed_kernel<RB, true>>();                                                                           \
-            transposed_kernel<RB, true><<<grid, THREADS, smem, st>>>(src, src_col_stride, dst, n, log_blowup, total_blocks, tw, ninv); \
-        } else {                                                                                                                  \
-            ensure_smem<transposed_kernel<RB, false>>();                                                                          \
-            transposed_kernel<RB, false><<<grid, THREADS, smem, st>>>(src, src_col_stride, dst, n, log_blowup, total_blocks, tw, ninv); \
-        }                                                                                                                         \
-        return true;                                                                                                              \
-    }
-    PB_CASE(8) PB_CASE(9) PB_CASE(10) PB_CASE(11) PB_CASE(12)
-#undef PB_CASE
-    return false;
-}
-
-inline bool supported(int n_hi, int n_lo) {
-    return n_hi >= 8 && n_hi <= 12 && (n_lo == n_hi || n_lo == n_hi + 1) && n_lo <= 12;     // 16 <= n <= 24
-}
+// Pass plan of a 2^n-point transform: n = n_hi + n_lo, K1/K3 = strided_kernel<n_hi, n_lo>, K2a/K2b = transposed_kernel<n_lo>.
+// Up to 2^10 points n_hi = 0: one transposed pass each way, then ntt::bitrev_store_kernel.
+constexpr int n_lo_of(int n) { return n <= 10 ? n : (n + 1) / 2; }
+// dynamic shared memory of a pass over 2^rb rows: at most 2^LOG_TILE words
+constexpr size_t tile_bytes(int rb) { return (size_t)4 << (rb + log_lc_of(rb)); }
 
 }  // namespace nttf

@@ -29,6 +29,7 @@ constexpr int RB = 10;                    // block = 2^10 positions
 constexpr int BLOCKS_PER_TILE = 16;       // 64 KB
 constexpr int THREADS = 256;              // 8 warps x 2 blocks
 constexpr uint32_t TILE_BYTES = BLOCKS_PER_TILE * (4u << RB);
+constexpr int SMEM_BYTES = TILE_BYTES + 1024;   // dynamic shared memory: the tile, aligned up to 1024 B in the kernel
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
@@ -162,23 +163,17 @@ inline bool make_map(CUtensorMap* tm, const uint32_t* base, size_t words) {
                        CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-// launches the TMA version of K2a / K2b; false when it does not apply (caller falls back to nttf::launch_transposed)
+// launches the TMA version of K2a / K2b; false when it does not apply (caller launches nttf::transposed_kernel instead).
+// The caller's context has opted both kernels in to SMEM_BYTES of dynamic shared memory.
 inline bool launch_transposed(bool inv, int n, int n_lo, cudaStream_t st, const uint32_t* src, uint32_t* dst, int log_blowup, size_t total_blocks,
                               size_t src_words, size_t dst_words, const uint2* tw, uint2 ninv) {
     if (!available() || !supported(n_lo) || (total_blocks % BLOCKS_PER_TILE) != 0 || (n - RB) < 4) return false;
     if ((src_words >> 5) > 0x7fffffffull || (dst_words >> 5) > 0x7fffffffull) return false;      // row coordinates are int32
     CUtensorMap ts, td;
     if (!make_map(&ts, src, src_words) || !make_map(&td, dst, dst_words)) return false;
-    static bool attr_done = false;
-    const size_t smem = TILE_BYTES + 1024;
-    if (!attr_done) {
-        cudaFuncSetAttribute(transposed_tma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        cudaFuncSetAttribute(transposed_tma_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        attr_done = true;
-    }
     const dim3 grid((unsigned)(total_blocks / BLOCKS_PER_TILE), 1, inv ? 1u : (1u << log_blowup));
-    if (inv) transposed_tma_kernel<true><<<grid, THREADS, smem, st>>>(ts, td, n, log_blowup, tw, ninv);
-    else transposed_tma_kernel<false><<<grid, THREADS, smem, st>>>(ts, td, n, log_blowup, tw, ninv);
+    if (inv) transposed_tma_kernel<true><<<grid, THREADS, SMEM_BYTES, st>>>(ts, td, n, log_blowup, tw, ninv);
+    else transposed_tma_kernel<false><<<grid, THREADS, SMEM_BYTES, st>>>(ts, td, n, log_blowup, tw, ninv);
     return true;
 }
 

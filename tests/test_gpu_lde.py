@@ -1,7 +1,7 @@
-"""Coset LDE (pb_lde_batch, pb_lde_shard) against the scalar oracle, every output word, at every compile-time specialised pass
-geometry (16 <= log_n <= 24: nttf::strided_kernel / transposed_kernel for (n_hi, n_lo) = (8,8) ... (12,12), and the TMA-staged
-transposed passes at n_lo = 10), with more than one coset, several column batches, twiddle-cache eviction, words at the edges of
-the lazy [0, 2p) arithmetic, and the row-sharded LDE.
+"""Coset LDE (pb_lde_batch, pb_lde_shard) against the scalar oracle, every output word, at every pass geometry (1 <= log_n <= 24:
+nttf::transposed_kernel alone up to 2^10, nttf::strided_kernel / transposed_kernel for (n_hi, n_lo) = (5,6) ... (12,12) above,
+and the TMA-staged transposed passes at n_lo = 10), with more than one coset, several column batches, twiddle-cache eviction,
+words at the edges of the lazy [0, 2p) arithmetic, and the row-sharded LDE.
 
 Device words are compared raw (Montgomery form) with the oracle's LDE converted to Montgomery form, so a kernel that leaves a
 word unreduced fails too.  Every output buffer starts as SENTINEL, which is not a valid Montgomery word, so a row the kernel
@@ -47,7 +47,8 @@ def random_shift(log_n):
 
 
 def n_lo_of(log_n):
-    """low split of the pass geometry, as make_geom in capi.cu: K2 blocks are 2^n_lo positions, K1/K3 lanes run over k mod 2^n_lo"""
+    """low split of the pass geometry, as nttf::n_lo_of in ntt_fast.cuh: K2 blocks are 2^n_lo positions, K1/K3 lanes run over
+    k mod 2^n_lo"""
     return log_n if log_n <= 10 else (log_n + 1) // 2
 
 
@@ -135,12 +136,14 @@ def refs(orc):
 
 
 # the geometry tests' trace at each size, and the references they take of it
+SMALL_SIZES = list(range(1, 16))        # n_hi = 0 up to 2^10, then (n_hi, n_lo) = (5,6) ... (7,8); every blow-up
 GEOM_SIZES = list(range(16, 25))
 BLOWUP_SIZES = [16, 19, 20, 24]         # n_lo = 8, 10 (TMA forward pass), 10 (TMA), 12
 
 
 def geom_width(log_n):
-    return 3 if log_n <= 21 else 2 if log_n <= 23 else 1
+    """up to 2^10 a column is one transposed block: 21 blocks leave 5 of the second CTA's 16 lanes live"""
+    return 21 if log_n <= 10 else 3 if log_n <= 21 else 2 if log_n <= 23 else 1
 
 
 def geom_shifts(log_n):
@@ -153,8 +156,13 @@ def geom_key(log_n, log_blowup, shift):
 
 def geom_ref(refs, log_n, log_blowup, shift):
     """the first request at a size computes all of that size's references: one per shift, at the largest blow-up asked for"""
-    top = {s: 3 if log_n in BLOWUP_SIZES and s != quotient_shift(log_n) else 1 for s in geom_shifts(log_n)}
-    return refs.get(geom_key(log_n, log_blowup, shift), [geom_key(log_n, b, s) for s, b in top.items()])
+    def top(s):
+        return 3 if log_n in SMALL_SIZES or (log_n in BLOWUP_SIZES and s != quotient_shift(log_n)) else 1
+    return refs.get(geom_key(log_n, log_blowup, shift), [geom_key(log_n, top(s), s) for s in geom_shifts(log_n)])
+
+
+def shift_of(kind, log_n):
+    return {"31": 31, "quotient": quotient_shift(log_n), "random": random_shift(log_n)}[kind]
 
 
 # ---------------------------------------------------------------- device calls
@@ -220,8 +228,19 @@ def test_reference_identities(orc):
 def test_lde_every_specialised_geometry_matches_oracle(ctx, refs, log_n, shift_kind):
     """(n_hi, n_lo) = (8,8) at 2^16 ... (12,12) at 2^24, full output; shifts 31, w_{2N}^{-1} (the prover's second quotient chunk)
     and a random one"""
-    shift = {"31": 31, "quotient": quotient_shift(log_n), "random": random_shift(log_n)}[shift_kind]
+    shift = shift_of(shift_kind, log_n)
     check_geom(ctx, refs, log_n, 1, shift, "blow-up 1, shift %d" % shift)
+
+
+@gpu
+@pytest.mark.parametrize("shift_kind", ["31", "quotient", "random"])
+@pytest.mark.parametrize("log_n", SMALL_SIZES)
+def test_lde_small_geometries_match_oracle(ctx, refs, log_n, shift_kind):
+    """2^1 ... 2^10: one transposed pass each way, then the bit-reversed store; 2^11 ... 2^15: (n_hi, n_lo) = (5,6) ... (7,8).
+    Blow-ups 1, 2 and 3, all from one 8-coset reference per shift"""
+    shift = shift_of(shift_kind, log_n)
+    for log_blowup in (1, 2, 3):
+        check_geom(ctx, refs, log_n, log_blowup, shift, "%d cosets, shift %d" % (1 << log_blowup, shift))
 
 
 # ---------------------------------------------------------------- 2. more than one coset on the specialised passes
@@ -280,7 +299,7 @@ def test_lde_at_reduction_edges_matches_oracle(ctx, orc, log_n):
 @gpu
 @pytest.mark.parametrize("batch", [1, 3, 5])
 @pytest.mark.parametrize("width", [7, 13])
-@pytest.mark.parametrize("log_n", [16, 20])
+@pytest.mark.parametrize("log_n", [9, 13, 16, 20])
 def test_lde_column_batches_match_oracle(ctx, refs, monkeypatch, log_n, width, batch):
     """PB_LDE_BATCH splits one call into ceil(width / batch) equal batches but the last (7 by 3: 3 + 3 + 1; 13 by 5: 5 + 5 + 3);
     4 cosets, so each batch writes its own slice of the output rows as well"""
@@ -338,10 +357,10 @@ def test_twiddle_cache_evicts_beyond_4_gib(refs):
 @gpu
 @pytest.mark.parametrize("shift_kind", ["31", "quotient"])
 @pytest.mark.parametrize("world", [2, 8])
-@pytest.mark.parametrize("log_n", [16, 20, 24])
+@pytest.mark.parametrize("log_n", [11, 16, 20, 24])
 def test_lde_shard_matches_oracle(ctx, refs, log_n, world, shift_kind):
     """pb_lde_shard block b = rows [b Ms, (b + 1) Ms) of the 2-coset LDE, Ms = 2N / world; its forward pass has 2^(n + 1 - g) rows,
-    g = log2(world): 2^14 (generic passes), 2^16, 2^18, 2^20, 2^22 and 2^24 (specialised)"""
+    g = log2(world): 2^9 (one transposed pass, then the bit-reversed store), 2^11, 2^14, 2^16, 2^18, 2^20, 2^22 and 2^24"""
     shift = 31 if shift_kind == "31" else quotient_shift(log_n)
     width = geom_width(log_n)
     exp = geom_ref(refs, log_n, 1, shift)
