@@ -151,8 +151,9 @@ int pb_prove_segment(pb_ctx_t* ctx, const pb_air_t* air, const uint32_t* trace, 
  *     when perm_width = 0) | quotient row (8) | quotient path (log_m x 8) | per FRI layer i: opened pair row (8), path ((log_m-1-i) x 8) ]
  * pb_last_openings: the opened values, [(width + 2*perm_width + 8)][4] canonical:
  *   main at zeta | perm at zeta | perm at zeta*w | quotient chunks at zeta. */
-/* ONE proof state per context: pb_prove_segment, pb_prove_segment_sharded and pb_prove_chips share workspaces, so each of them invalidates
- * the query state of any earlier proof of the context (a later pb_query_* / pb_last_openings for it returns PB_ERR_INVALID_ARG). */
+/* ONE proof state per context: pb_prove_segment, pb_prove_segment_sharded and pb_prove_chips share workspaces, so each of them, even when
+ * it fails, invalidates the query state of any earlier proof of the context; each pb_query_* answers only for a proof of its own prover,
+ * pb_last_openings for pb_prove_segment and pb_prove_segment_sharded (otherwise they return PB_ERR_INVALID_ARG). */
 int pb_query_words(size_t log_n, size_t width, size_t perm_width, size_t* words_per_query);
 int pb_query_segment(pb_ctx_t* ctx, uint32_t* h_out, size_t out_capacity_words);
 int pb_last_openings(pb_ctx_t* ctx, uint32_t* h_ys, size_t capacity_words);
@@ -238,8 +239,9 @@ int pb_query_segment_sharded(pb_ctx_t* ctx, const pb_comm_t* comm, uint32_t* h_o
  * times with the default constants, canonical words in and out, without a device: a known-answer / cross-check hook. */
 int pb_host_poseidon2_permute(uint32_t state[16], int reps, int force_scalar, int* used_avx512);
 
-/* per-stage device milliseconds of the last pb_prove_segment:
- * [h2d, lde, merkle, logup_gen, logup_commit, quotient, qlde, qmerkle, open, fri, pow, total] */
+/* per-stage device milliseconds of the last pb_prove_segment, pb_prove_chips or pb_prove_segment_sharded:
+ * [h2d, lde, merkle, logup_gen, logup_commit, quotient, qlde, qmerkle, open, fri, pow, total]; for several chips a stage spans that
+ * phase of every chip (pb_prove_chips runs each phase for all chips before the next). */
 #define PB_N_STAGES 12
 int pb_last_stage_ms(pb_ctx_t* ctx, float ms[PB_N_STAGES]);
 /* kernels launched by this context since creation (bench.py's gpu_launches) */

@@ -145,7 +145,8 @@ struct pb_bus {
     std::vector<unsigned> grid_y;
 };
 
-// one chip of a multi-chip segment (chips.inl): its matrices stay resident between pb_prove_chips and pb_query_chips
+// one chip of a proof (chips.inl): its matrices stay resident until the query phase.  pb_prove_segment and pb_prove_segment_sharded
+// use slot 0 (the sharded prover holds its row blocks there).
 struct McChip {
     size_t log_n = 0, width = 0, wp = 0, n_chunks = 0, e_main = 0, e_perm = 0, e_q = 0;
     const pb_air* air = nullptr;
@@ -165,50 +166,36 @@ struct pb_ctx {
     int fold_tab_log_len = 0;
     DevBuf<uint32_t> tmp, tmp2;       // LDE intermediates (L2-sized)
     DevBuf<const uint32_t*> coltab;
-    // pb_prove_segment workspace
-    DevBuf<uint32_t> ws_trace, ws_lde, ws_layers, ws_q, ws_qnat, ws_qlde, ws_f0, ws_state, ws_ys;
+    // proof workspaces: the matrices of every prover live in the chip slots and the three trees
+    std::vector<McChip> chips;
+    DevBuf<uint32_t> tree_main, tree_perm, tree_q;   // main, permutation and quotient commitments (node-major layers)
+    DevBuf<uint32_t> ro[32];                         // reduced-opening codeword of each LDE height below the tallest
+    DevBuf<uint32_t> ws_trace, ws_q, ws_f0, ws_state, ws_ys;
     DevBuf<uint4> ws_w, ws_part;          // barycentric weights [N], per-CTA partial sums of the openings
     DevBuf<uint2> ws_gp;                  // gamma powers of the reduced opening, canonical (one uint4 per column)
-    DevBuf<uint32_t> ws_layers_q, ws_fri_words, ws_fri_trees, ws_qidx, ws_qout;
+    DevBuf<uint32_t> ws_fri_words, ws_fri_trees, ws_qidx, ws_qout;
     DevBuf<uint32_t> ws_shard_send, ws_shard_recv, ws_shard_coef, ws_gather, ws_gather2;   // multi-GPU segment (shard_api.inl)
     DevBuf<uint32_t> ws_qraw;             // running constraint fold between the chunks of a JIT-compiled AIR, [4][rows]
-    DevBuf<uint32_t> ws_perm, ws_perm_lde, ws_layers_p, ws_rowsum, ws_scan_tot, ws_lu_raw, ws_lu_s, ws_pow;   // LogUp phase + PoW
+    DevBuf<uint32_t> ws_rowsum, ws_scan_tot, ws_lu_raw, ws_lu_s, ws_pow;   // LogUp phase + PoW
+    DevBuf<uint32_t> ws_mc_dig;           // digests of the shorter height groups until the tree reaches their level
     uint32_t n_queries = 100, pow_bits = 16;
-    // what pb_query_segment needs from the last pb_prove_segment (everything stays resident on the device)
-    struct {
-        bool valid = false;
-        size_t log_n = 0, log_m = 0, width = 0, perm_width = 0;
-        uint32_t n_layers = 0;
-        size_t word_off[32] = {0}, tree_off[32] = {0};
-        Challenger ch;                       // transcript state after the FRI commit phase
-        std::vector<uint32_t> ys;            // opened values, Montgomery, [(width + 2 perm_width + 8)][4]
-    } seg;
     DevBuf<uint32_t> ws_fri_ch, ws_fri_log;  // device challenger state and the (root, beta) log of the FRI commit phase
-    // what pb_query_segment_sharded needs from the last pb_prove_segment_sharded: this rank's row blocks and subtrees stay resident
-    // (ws_lde / ws_perm_lde / ws_qlde, ws_layers*), the FRI layers in ws_fri_words / ws_fri_trees, every tree's G subtree roots here
+    DevBuf<uint32_t> ws_sh_q, ws_sh_qall;    // this rank's share of the query openings, and all ranks' shares
+    // The last proof, read by the query phase of the prover that made it (everything else stays resident on the device).
+    enum class Prover { segment, chips, sharded };
     struct {
         bool valid = false;
-        size_t log_n = 0, width = 0, perm_width = 0;
-        int G = 0, g = 0, rank = 0;
+        Prover by = Prover::segment;
+        size_t K = 0, hmax = 0, hperm = 0;   // chips; log2 of the tallest LDE, of the tallest one with a permutation trace
         uint32_t n_layers = 0;
-        bool layer_sharded[33] = {false};
         size_t word_off[33] = {0}, tree_off[33] = {0};
+        Challenger ch;                       // transcript state after the proof of work
+        std::vector<uint32_t> ys;            // opened values, Montgomery, [n_opened][4]
+        // pb_prove_segment_sharded: which FRI layers are row-sharded, every tree's G subtree roots
+        int G = 0, g = 0, rank = 0;
+        bool layer_sharded[33] = {false};
         uint32_t roots_main[16][8], roots_perm[16][8], roots_q[16][8], roots_fri[32][16][8];   // Montgomery
-        Challenger ch;
-    } sh;
-    DevBuf<uint32_t> ws_sh_q, ws_sh_qall;    // this rank's share of the query openings, and all ranks' shares
-    // multi-chip segment (chips.inl)
-    DevBuf<uint32_t> ws_mc_dig;              // digests of the shorter height groups until the tree reaches their level
-    struct {
-        bool valid = false, any_lu = false;
-        size_t K = 0, hmax = 0, hperm = 0;
-        uint32_t n_layers = 0;
-        size_t word_off[32] = {0}, tree_off[32] = {0};
-        Challenger ch;
-        std::vector<uint32_t> ys;
-        std::vector<McChip> chips;
-        DevBuf<uint32_t> tree_main, tree_perm, tree_q, ro[32];
-    } mc;
+    } last;
     cudaStream_t copy_stream = nullptr;   // H2D chunks of the host-input pipeline
     cudaStream_t lde_streams[8] = {nullptr};   // PB_LDE_STREAMS experiment
     cudaEvent_t lde_join[8] = {nullptr}, lde_fork = nullptr;
@@ -351,6 +338,27 @@ int read_root(pb_ctx* ctx, const uint32_t* d_layers, size_t log_h, uint32_t root
     const size_t root_off = 8 * (((size_t)2 << log_h) - 2);
     CK(cudaMemcpyAsync(root_m, d_layers + root_off, 32, cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
+    return 0;
+}
+
+// leaf digests of 2^log_h rows over the column-major columns `cols` into d_out (8 words per row), timed for pb_leaf_kernel_profile
+int leaf_hash_cols(pb_ctx* ctx, const std::vector<const uint32_t*>& cols, size_t log_h, uint32_t* d_out) {
+    const size_t h = (size_t)1 << log_h;
+    RC(ctx->coltab.ensure(std::max<size_t>(1, cols.size())));
+    // (pageable source: staged before the call returns; the table itself is reused in stream order)
+    CK(cudaMemcpyAsync(ctx->coltab.p, cols.data(), cols.size() * sizeof(void*), cudaMemcpyHostToDevice, ctx->stream));
+    const int slot = ctx->kp_n < pb_ctx::KPROF ? ctx->kp_n : -1;
+    if (slot >= 0) CK(cudaEventRecord(ctx->kp_a[slot], ctx->stream));
+    if (h <= LEAF_COOP)
+        p2::leaf_hash_cols_coop_kernel<<<(unsigned)((16 * h + 255) / 256), 256, 0, ctx->stream>>>(ctx->coltab.p, (uint32_t)cols.size(), h, d_out);
+    else
+        p2::leaf_hash_cols_kernel<<<(unsigned)((h + p2::LEAF_THREADS - 1) / p2::LEAF_THREADS), p2::LEAF_THREADS, 0, ctx->stream>>>(ctx->coltab.p, (uint32_t)cols.size(), h, d_out);
+    LAUNCHED(ctx);
+    if (slot >= 0) {
+        CK(cudaEventRecord(ctx->kp_b[slot], ctx->stream));
+        ctx->kp_bytes[slot] = 4.0 * (double)h * (double)cols.size() + 32.0 * (double)h;   // algorithmic bytes: matrix in, digests out
+        ctx->kp_n++;
+    }
     return 0;
 }
 
@@ -781,21 +789,8 @@ int pb_merkle_commit(pb_ctx_t* ctx, const uint32_t* const* d_mats, const size_t*
     std::vector<const uint32_t*> cols;
     for (size_t i = 0; i < n_mats; i++)
         for (size_t c = 0; c < widths[i]; c++) cols.push_back(d_mats[i] + c * h);
-    int rc = ctx->coltab.ensure(std::max<size_t>(1, cols.size()));
+    int rc = leaf_hash_cols(ctx, cols, log_h, d_layers);
     if (rc) return rc;
-    CK(cudaMemcpyAsync(ctx->coltab.p, cols.data(), cols.size() * sizeof(void*), cudaMemcpyHostToDevice, ctx->stream));
-    const int slot = ctx->kp_n < pb_ctx::KPROF ? ctx->kp_n : -1;
-    if (slot >= 0) CK(cudaEventRecord(ctx->kp_a[slot], ctx->stream));
-    if (h <= LEAF_COOP)
-        p2::leaf_hash_cols_coop_kernel<<<(unsigned)((16 * h + 255) / 256), 256, 0, ctx->stream>>>(ctx->coltab.p, (uint32_t)cols.size(), h, d_layers);
-    else
-        p2::leaf_hash_cols_kernel<<<(unsigned)((h + p2::LEAF_THREADS - 1) / p2::LEAF_THREADS), p2::LEAF_THREADS, 0, ctx->stream>>>(ctx->coltab.p, (uint32_t)cols.size(), h, d_layers);
-    LAUNCHED(ctx);
-    if (slot >= 0) {
-        CK(cudaEventRecord(ctx->kp_b[slot], ctx->stream));
-        ctx->kp_bytes[slot] = 4.0 * (double)h * (double)cols.size() + 32.0 * (double)h;   // algorithmic bytes: matrix in, digests out
-        ctx->kp_n++;
-    }
     rc = merkle_upper(ctx, d_layers, log_h);
     if (rc) return rc;
     if (root_out) {
@@ -950,49 +945,44 @@ static int eval_at_point_m(pb_ctx* ctx, const uint32_t* d_mat, size_t log_n, siz
     return 0;
 }
 
-// reduced opening over shift*H' (bit-reversed rows).  `cols[j]` is opened at point zs[grp[j]]; its gamma exponent is j (the order
-// in which the opened values are observed).  ys_m: host, [n_cols][4] Montgomery.  One kernel launch per point (the later ones
-// accumulate into d_out).  rows [row0, row0 + n_rows) of the domain only when n_rows != 0 (cols[] then point at that row block).
-// gamma_start (optional): gamma exponent of cols[0] as a power already computed (multi-chip prover: a chip's block starts at its
-// position in the observation order); accumulate: add to d_out instead of overwriting it.
-static int deep_quotient_groups_m(pb_ctx* ctx, const std::vector<const uint32_t*>& cols, const std::vector<uint32_t>& grp, const std::vector<bb::E4>& zs,
-                                  size_t log_m, uint32_t shift_m, bb::E4 gamma_m, const uint32_t* ys_m, uint32_t* d_out, size_t row0 = 0, size_t n_rows = 0,
-                                  const bb::E4* gamma_start = nullptr, bool accumulate = false) {
+// reduced opening over shift*H' (bit-reversed rows).  `cols[j]` is opened at point zs[grp[j]]; e[j] is its position in the order in
+// which the opened values are observed: its gamma exponent and the index of its value in ys_m (host, [..][4] Montgomery).  Rows
+// [row0, row0 + n_rows) of the domain only when n_rows != 0 (cols[] then point at that row block).
+// Columns of group 0 go in runs of equal stride; a run of group-1 columns that repeats a group-0 run (same base, stride, count: the
+// permutation trace opened at zeta and at zeta*w) is attached to it, so those columns are read from HBM once.  One launch per
+// DQ_MAX_SEGS runs: the first writes d_out, the later ones add to it.
+static int deep_quotient_groups_m(pb_ctx* ctx, const std::vector<const uint32_t*>& cols, const std::vector<uint32_t>& grp, const std::vector<uint32_t>& e,
+                                  const std::vector<bb::E4>& zs, size_t log_m, uint32_t shift_m, bb::E4 gamma_m, const uint32_t* ys_m, uint32_t* d_out,
+                                  size_t row0 = 0, size_t n_rows = 0) {
     const size_t n_cols = cols.size(), M = n_rows ? n_rows : (size_t)1 << log_m;
-    if (n_cols == 0 || grp.size() != n_cols) return PB_ERR_INVALID_ARG;
+    if (n_cols == 0 || grp.size() != n_cols || e.size() != n_cols || zs.empty()) return PB_ERR_INVALID_ARG;
+    if (zs.size() > 2) return PB_ERR_UNSUPPORTED;
+    std::vector<bb::E4> gp(n_cols);                   // gamma^e[j]: one product along a run of consecutive exponents
     std::vector<uint4> gs(n_cols);
-    std::vector<bb::E4> ysum(zs.size(), bb::E4{{0u, 0u, 0u, 0u}});
-    bb::E4 cur = gamma_start ? *gamma_start : bb::E4{{bb::R1, 0u, 0u, 0u}};
     for (size_t j = 0; j < n_cols; j++) {
-        uint32_t c[4];
-        for (int l = 0; l < 4; l++) c[l] = h_from_m(cur.c[l]);
-        gs[j] = make_uint4(c[0], c[1], c[2], c[3]);
-        bb::E4 y;
-        memcpy(y.c, ys_m + 4 * j, 16);
-        ysum[grp[j]] = bb::e4_add(ysum[grp[j]], bb::e4_mul(cur, y));
-        cur = bb::e4_mul(cur, gamma_m);
+        if (grp[j] >= zs.size()) return PB_ERR_INVALID_ARG;
+        if (j && e[j] == e[j - 1] + 1) {
+            gp[j] = bb::e4_mul(gp[j - 1], gamma_m);
+        } else {
+            bb::E4 r = {{bb::R1, 0u, 0u, 0u}}, base = gamma_m;
+            for (uint32_t x = e[j]; x; x >>= 1) { if (x & 1) r = bb::e4_mul(r, base); base = bb::e4_mul(base, base); }
+            gp[j] = r;
+        }
+        gs[j] = make_uint4(h_from_m(gp[j].c[0]), h_from_m(gp[j].c[1]), h_from_m(gp[j].c[2]), h_from_m(gp[j].c[3]));
     }
     int rc = ctx->ws_gp.ensure(2 * n_cols);          // uint2 elements: one uint4 per column
     if (rc) return rc;
     CK(cudaMemcpyAsync(ctx->ws_gp.p, gs.data(), gs.size() * sizeof(uint4), cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));           // gs is a host temporary
-    // one launch: columns of group 0 in runs of equal stride; a run of group-1 columns that repeats a group-0 run (same base, stride,
-    // count: the permutation trace opened at zeta and at zeta*w) is attached to it, so those columns are read from HBM once
-    if (zs.size() > 2) return PB_ERR_UNSUPPORTED;
-    deep::DeepSegs segs{};
+    struct Run { const uint32_t* base; size_t stride; uint32_t count, off, off2; };
+    std::vector<Run> runs;
     for (size_t j = 0; j < n_cols;) {
         if (grp[j] != 0) { j++; continue; }
-        if (segs.n == deep::DQ_MAX_SEGS) return PB_ERR_UNSUPPORTED;
         size_t k = j + 1;
         const ptrdiff_t st = (k < n_cols && grp[k] == 0) ? cols[k] - cols[j] : 0;
         while (k < n_cols && grp[k] == 0 && st > 0 && cols[k] - cols[k - 1] == st) k++;
         if (st <= 0) k = j + 1;
-        segs.base[segs.n] = cols[j];
-        segs.stride[segs.n] = st > 0 ? (size_t)st : 0;
-        segs.count[segs.n] = (uint32_t)(k - j);
-        segs.gp_off[segs.n] = (uint32_t)j;
-        segs.gp_off2[segs.n] = deep::DQ_NO_SECOND;
-        segs.n++;
+        runs.push_back(Run{cols[j], st > 0 ? (size_t)st : 0, (uint32_t)(k - j), (uint32_t)j, deep::DQ_NO_SECOND});
         j = k;
     }
     for (size_t j = 0; j < n_cols;) {           // group-1 runs must mirror a group-0 run
@@ -1000,22 +990,46 @@ static int deep_quotient_groups_m(pb_ctx* ctx, const std::vector<const uint32_t*
         size_t k = j + 1;
         while (k < n_cols && grp[k] == 1) k++;
         bool placed = false;
-        for (int sgi = 0; sgi < segs.n && !placed; sgi++)
-            if (segs.base[sgi] == cols[j] && segs.count[sgi] == (uint32_t)(k - j) && segs.gp_off2[sgi] == deep::DQ_NO_SECOND &&
-                (k - j < 2 || (size_t)(cols[j + 1] - cols[j]) == segs.stride[sgi])) {
+        for (size_t sgi = 0; sgi < runs.size() && !placed; sgi++) {
+            Run& r = runs[sgi];
+            if (r.base == cols[j] && r.count == (uint32_t)(k - j) && r.off2 == deep::DQ_NO_SECOND && (k - j < 2 || (size_t)(cols[j + 1] - cols[j]) == r.stride)) {
                 bool same = true;
-                for (size_t t = j; t < k && same; t++) same = cols[t] == segs.base[sgi] + (t - j) * segs.stride[sgi];
-                if (same) { segs.gp_off2[sgi] = (uint32_t)j; placed = true; }
+                for (size_t t = j; t < k && same; t++) same = cols[t] == r.base + (t - j) * r.stride;
+                if (same) { r.off2 = (uint32_t)j; placed = true; }
             }
+        }
         if (!placed) return PB_ERR_UNSUPPORTED;
         j = k;
     }
-    const bool two = zs.size() == 2;
-    deep::deep_quotient_kernel<<<(unsigned)((M + 255) / 256), 256, 0, ctx->stream>>>(segs, M, (int)log_m, row0, shift_m, h_root_of_unity_m((int)log_m),
-                                                                                    reinterpret_cast<const uint4*>(ctx->ws_gp.p), ysum[0], zs[0],
-                                                                                    two ? ysum[1] : ysum[0], two ? zs[1] : zs[0], two ? 1 : 0,
-                                                                                    reinterpret_cast<uint4*>(d_out), accumulate ? 1 : 0);
-    LAUNCHED(ctx);
+    for (size_t r0 = 0; r0 < runs.size(); r0 += deep::DQ_MAX_SEGS) {
+        deep::DeepSegs segs{};
+        bb::E4 ysum[2] = {{{0u, 0u, 0u, 0u}}, {{0u, 0u, 0u, 0u}}};      // sum of gamma^e[j] y_j over this launch's columns, per point
+        auto add_y = [&](int pt, size_t j) {
+            bb::E4 y;
+            memcpy(y.c, ys_m + 4 * (size_t)e[j], 16);
+            ysum[pt] = bb::e4_add(ysum[pt], bb::e4_mul(gp[j], y));
+        };
+        bool two = false;
+        for (size_t i = r0; i < std::min(runs.size(), r0 + deep::DQ_MAX_SEGS); i++) {
+            const Run& r = runs[i];
+            segs.base[segs.n] = r.base;
+            segs.stride[segs.n] = r.stride;
+            segs.count[segs.n] = r.count;
+            segs.gp_off[segs.n] = r.off;
+            segs.gp_off2[segs.n] = r.off2;
+            segs.n++;
+            for (uint32_t t = 0; t < r.count; t++) add_y(0, r.off + t);
+            if (r.off2 != deep::DQ_NO_SECOND) {
+                two = true;
+                for (uint32_t t = 0; t < r.count; t++) add_y(1, r.off2 + t);
+            }
+        }
+        deep::deep_quotient_kernel<<<(unsigned)((M + 255) / 256), 256, 0, ctx->stream>>>(segs, M, (int)log_m, row0, shift_m, h_root_of_unity_m((int)log_m),
+                                                                                        reinterpret_cast<const uint4*>(ctx->ws_gp.p), ysum[0], zs[0],
+                                                                                        two ? ysum[1] : ysum[0], two ? zs[1] : zs[0], two ? 1 : 0,
+                                                                                        reinterpret_cast<uint4*>(d_out), r0 > 0 ? 1 : 0);
+        LAUNCHED(ctx);
+    }
     CK(cudaGetLastError());
     return 0;
 }
@@ -1035,7 +1049,9 @@ int pb_deep_quotient(pb_ctx_t* ctx, const uint32_t* const* d_mats, const size_t*
     std::vector<uint32_t> ys(4 * cols.size());
     CK(cudaMemcpyAsync(ys.data(), d_ys, 16 * cols.size(), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
-    return deep_quotient_groups_m(ctx, cols, std::vector<uint32_t>(cols.size(), 0u), {h_e4_from_canon(zeta)}, log_m, h_to_m(shift),
+    std::vector<uint32_t> e(cols.size());
+    for (size_t j = 0; j < e.size(); j++) e[j] = (uint32_t)j;
+    return deep_quotient_groups_m(ctx, cols, std::vector<uint32_t>(cols.size(), 0u), e, {h_e4_from_canon(zeta)}, log_m, h_to_m(shift),
                                   h_e4_from_canon(gamma), ys.data(), d_out);
 }
 

@@ -43,6 +43,7 @@ def _gpu_prove(ctx, chips):
     [(4, 9, 3, 0), (4, 5, 2, 0)],                                       # no interactions anywhere: no permutation commitment
     [(3, 10, 0, 3), (7, 8, 2, 0)],                                      # the tallest chip is not the first and has no interactions
     [(8, 6, 2, 4), (8, 7, 0, 3), (8, 5, 1, 0)],                         # equal heights: one leaf row over all matrices
+    [(4, 6, 1, 2), (4, 5, 0, 3), (4, 7, 2, 1), (4, 4, 1, 2), (4, 6, 0, 2)],   # 15 column runs at one height: a split reduced opening
 ])
 def test_chips_proof_matches_oracle_bit_for_bit(ctx, orc, spec):
     chips = _chips(spec, seed=len(spec))
@@ -69,6 +70,9 @@ def test_one_chip_equals_the_single_chip_prover(ctx, orc):
     assert proof["quotient_root"] == single["quotient_root"] and proof["fri_roots"] == single["fri_roots"]
     assert proof["pow_witness"] == single["pow_witness"] and (ys == ys1).all() and (q == q1).all()
     assert cs[0].tolist() == single["cumulative_sum"]
+    shared = set(proof) & set(single)                   # every other field of the one-chip proof keeps its name
+    assert len(shared) >= 14 and {k: proof[k] for k in shared} == {k: single[k] for k in shared}
+    assert single["perm_width"] == air.perm_width
 
 
 def test_satisfying_traces_verify_with_the_constraint_identity(ctx, orc):
@@ -94,6 +98,38 @@ def test_chips_at_scale_verify(ctx, orc):
     assert orc.verify_chips(small, *p_small, check_constraints=False) == 0
     again = _gpu_prove(ctx, chips)
     assert again[0] == proof and (again[3] == q).all()
+
+
+@pytest.mark.parametrize("first", ["chips", "segment", "failed_segment"])
+def test_a_query_reads_only_the_proof_of_its_own_prover(ctx, first):
+    """the context keeps one proof state: after a proof by another prover, or after a failed proof, a query is refused; a proof by the
+    query's own prover makes it answer again"""
+    import ctypes as C
+    from powdr_b200.capi import SegmentProof
+    lib = ctx.lib
+    chips = _chips([(5, 12, 4, 5), (3, 8, 3, 0)], seed=4)
+    trace, bc, spans, bus = chips[0]
+    air = ctx.air(bc, spans, trace.shape[0], bus)
+    d = ctx.to_device(trace)
+    out = np.zeros(1 << 20, dtype=np.uint32)
+    ptr, cap = out.ctypes.data_as(C.c_void_p), C.c_size_t(out.size)
+    if first == "chips":
+        _gpu_prove(ctx, chips)
+        assert lib.pb_query_segment(ctx.h, ptr, cap) == -1
+        assert lib.pb_last_openings(ctx.h, ptr, cap) == -1
+    elif first == "segment":
+        ctx.prove_segment(air, d.ptr, 5, trace.shape[0], on_device=True)
+        assert lib.pb_query_chips(ctx.h, ptr, cap, None, C.c_size_t(0)) == -1
+        _gpu_prove(ctx, chips)                          # queries its own proof (pb_query_chips) or raises
+    else:
+        ctx.prove_segment(air, d.ptr, 5, trace.shape[0], on_device=True)
+        bad = lib.pb_prove_segment(ctx.h, air.h, C.c_void_p(d.ptr), C.c_size_t(5), C.c_size_t(trace.shape[0] + 1), C.c_uint32(1), C.byref(SegmentProof()))
+        assert bad == -1
+        assert lib.pb_query_segment(ctx.h, ptr, cap) == -1
+    if first != "segment":
+        ctx.prove_segment(air, d.ptr, 5, trace.shape[0], on_device=True)
+        ctx.query_segment(5, trace.shape[0], air.perm_width)      # raises unless both the query and the opened values are returned
+    air.free()
 
 
 def test_argument_checks(ctx):
