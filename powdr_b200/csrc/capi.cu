@@ -180,7 +180,7 @@ struct pb_ctx {
     DevBuf<uint32_t> ws_mc_dig;           // digests of the shorter height groups until the tree reaches their level
     uint32_t n_queries = 100, pow_bits = 16;
     DevBuf<uint32_t> ws_fri_ch, ws_fri_log;  // device challenger state and the (root, beta) log of the FRI commit phase
-    DevBuf<uint32_t> ws_sh_q, ws_sh_qall;    // this rank's share of the query openings, and all ranks' shares
+    DevBuf<uint32_t> ws_sh_qall;             // every rank's share of the query openings
     // The last proof, read by the query phase of the prover that made it (everything else stays resident on the device).
     enum class Prover { segment, chips, sharded };
     struct {
@@ -191,16 +191,18 @@ struct pb_ctx {
         size_t word_off[33] = {0}, tree_off[33] = {0};
         Challenger ch;                       // transcript state after the proof of work
         std::vector<uint32_t> ys;            // opened values, Montgomery, [n_opened][4]
-        // pb_prove_segment_sharded: which FRI layers are row-sharded, every tree's G subtree roots
-        int G = 0, g = 0, rank = 0;
+        // The context holds row block `rank` of G = 2^g of every committed matrix with the subtree over it, and of every row-sharded
+        // FRI layer; a replicated layer is held whole by rank 0.  One GPU: G = 1.  top_*: the tree over each commitment's G subtree
+        // roots, node-major like every tree (2G - 1 nodes, Montgomery)
+        int G = 1, g = 0, rank = 0;
         bool layer_sharded[33] = {false};
-        uint32_t roots_main[16][8], roots_perm[16][8], roots_q[16][8], roots_fri[32][16][8];   // Montgomery
+        uint32_t top_main[31][8], top_perm[31][8], top_q[31][8], top_fri[32][31][8];
     } last;
     cudaStream_t copy_stream = nullptr;   // H2D chunks of the host-input pipeline
     cudaStream_t lde_streams[8] = {nullptr};   // PB_LDE_STREAMS experiment
     cudaEvent_t lde_join[8] = {nullptr}, lde_fork = nullptr;
     cudaEvent_t ev_copy[2] = {nullptr}, ev_free[2] = {nullptr};
-    cudaEvent_t ev[16] = {nullptr};
+    cudaEvent_t ev[12] = {nullptr};         // stage boundaries of pb_last_stage_ms (stage_clocks)
     float stage_ms[PB_N_STAGES] = {0};     // h2d, lde, merkle, logup_gen, logup_commit, quotient, qlde, qmerkle, open(+deep), fri, pow, total
     // live timing of the dominant kernel (Poseidon2 leaf hashing over column-major matrices): event pairs on the stream
     static constexpr int KPROF = 16;
@@ -855,13 +857,14 @@ int pb_fri_fold(pb_ctx_t* ctx, const uint32_t* d_in, size_t log_len, uint32_t sh
     return fri_fold_m(ctx, d_in, log_len, h_to_m(shift), h_e4_from_canon(beta), d_out);
 }
 
-// FRI commit phase, device-driven: the codeword at ws_fri_words[0 .. 4 * 2^log_len0) is committed and folded down to length 2 without
-// a host round trip per layer (p2::fri_challenge_kernel keeps the duplex state on the device and hands the challenge to the fold
-// through memory).  Layer codewords / trees stay in ws_fri_words / ws_fri_trees at word_off / tree_off for the query phase.
+// FRI commit phase, device-driven: from layer `layer0`, whose codeword of length 2^log_len0 is at ws_fri_words + word_off[layer0] and
+// whose tree goes to ws_fri_trees + tree_off[layer0], the codeword is committed and folded down to length 2 without a host round trip
+// per layer (p2::fri_challenge_kernel keeps the duplex state on the device and hands the challenge to the fold through memory).  Layer
+// codewords / trees stay in ws_fri_words / ws_fri_trees, which the caller has sized, at word_off / tree_off for the query phase.
 // inject (optional, [32]): inject[h] is added to the folded codeword when it reaches length 2^h (multi-chip segments).
 // Afterwards ONE read-back of (roots, challenges, final values) and the host replays the transcript: `ch` advances exactly as if
 // it had driven the phase, and any difference from what the device sampled is PB_ERR_INTERNAL.
-static int fri_commit_phase(pb_ctx* ctx, Challenger& ch, size_t log_len0, uint32_t* const* inject, size_t* word_off, size_t* tree_off,
+static int fri_commit_phase(pb_ctx* ctx, Challenger& ch, uint32_t layer0, size_t log_len0, uint32_t* const* inject, size_t* word_off, size_t* tree_off,
                             uint32_t* n_layers, uint32_t fri_roots[32][8], uint32_t fri_betas[32][4], uint32_t fin_m[8], cudaEvent_t after_last_kernel) {
     cudaStream_t st = ctx->stream;
     int rc;
@@ -871,9 +874,10 @@ static int fri_commit_phase(pb_ctx* ctx, Challenger& ch, size_t log_len0, uint32
     if ((rc = get_fold_table(ctx, (int)log_len0))) return rc;
     uint32_t* d_sponge = ctx->ws_fri_ch.p;
     CK(cudaMemcpyAsync(d_sponge, ch.sponge, 64, cudaMemcpyHostToDevice, st));    // pageable source: staged before the call returns
-    uint32_t* f = ctx->ws_fri_words.p;
-    size_t log_len = log_len0, woff = 0, toff = 0;
-    uint32_t shift_m = h_to_m(bb::GEN), layer = 0;
+    size_t log_len = log_len0, woff = word_off[layer0], toff = tree_off[layer0];
+    uint32_t* f = ctx->ws_fri_words.p + woff;
+    uint32_t shift_m = h_to_m(bb::GEN), layer = layer0;
+    for (uint32_t l = 0; l < layer0; l++) shift_m = bb::mul(shift_m, shift_m);
     const uint32_t two_inv = bb::inv(h_to_m(2));
     while (log_len > 1) {
         uint32_t* tree = ctx->ws_fri_trees.p + toff;
@@ -902,10 +906,10 @@ static int fri_commit_phase(pb_ctx* ctx, Challenger& ch, size_t log_len0, uint32
     CK(cudaGetLastError());
     uint32_t log_h[32 * 12];
     CK(cudaMemcpyAsync(fin_m, f, 32, cudaMemcpyDeviceToHost, st));
-    if (layer) CK(cudaMemcpyAsync(log_h, ctx->ws_fri_log.p, 48 * (size_t)layer, cudaMemcpyDeviceToHost, st));
+    if (layer > layer0) CK(cudaMemcpyAsync(log_h + 12 * layer0, ctx->ws_fri_log.p + 12 * layer0, 48 * (size_t)(layer - layer0), cudaMemcpyDeviceToHost, st));
     if (after_last_kernel) CK(cudaEventRecord(after_last_kernel, st));
     CK(cudaStreamSynchronize(st));
-    for (uint32_t l = 0; l < layer; l++) {
+    for (uint32_t l = layer0; l < layer; l++) {
         ch.observe(log_h + 12 * l, 8);
         const bb::E4 beta = ch.sample_ext();
         if (memcmp(beta.c, log_h + 12 * l + 8, 16) != 0) return PB_ERR_INTERNAL;

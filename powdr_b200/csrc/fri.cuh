@@ -47,6 +47,8 @@ __global__ void __launch_bounds__(256) add_words_kernel(uint32_t* __restrict__ f
 // One CTA per query and one launch per piece of the layout (include/powdr_b200.h): the index; per commitment the row of each of its
 // matrices, then the Merkle path; per FRI layer i the opened pair and its path ((log_max-1-i) x 8).  All words canonical.
 // Merkle trees are node-major with level k at node offset 2^(h+1) - 2^(h-k+1); the sibling of leaf idx at level k is (idx>>k)^1.
+// A context gathers what it holds: a window of rows [row0, row0 + rows) of each matrix (stored with stride rows) and the subtree over
+// them, which gives the bottom log2(rows) levels of the path.  A query whose row lies outside the window writes nothing.
 namespace fri {
 
 __device__ __forceinline__ void copy_path(const uint32_t* tree, int log_h, size_t idx, uint32_t* out) {
@@ -57,32 +59,40 @@ __device__ __forceinline__ void copy_path(const uint32_t* tree, int log_h, size_
     }
 }
 
-// out[q * wpq + off + c] = canonical(mat[c * m + (idx[q] >> shift)])
-__global__ void gather_rows_kernel(const uint32_t* __restrict__ mat, size_t m, uint32_t width, int shift, const uint32_t* __restrict__ idx, uint32_t* __restrict__ out,
-                                   size_t wpq, size_t off) {
-    const size_t r = idx[blockIdx.x] >> shift;
+// out[q * wpq + off + c] = canonical(mat[c * rows + (idx[q] >> shift) - row0])
+__global__ void gather_rows_kernel(const uint32_t* __restrict__ mat, size_t row0, size_t rows, uint32_t width, int shift, const uint32_t* __restrict__ idx,
+                                   uint32_t* __restrict__ out, size_t wpq, size_t off) {
+    const size_t r = (idx[blockIdx.x] >> shift) - row0;
+    if (r >= rows) return;
     uint32_t* o = out + (size_t)blockIdx.x * wpq + off;
-    for (uint32_t c = threadIdx.x; c < width; c += blockDim.x) o[c] = bb::from_monty(mat[(size_t)c * m + r]);
+    for (uint32_t c = threadIdx.x; c < width; c += blockDim.x) o[c] = bb::from_monty(mat[(size_t)c * rows + r]);
 }
-__global__ void gather_path_kernel(const uint32_t* __restrict__ tree, int log_h, int shift, const uint32_t* __restrict__ idx, uint32_t* __restrict__ out, size_t wpq,
-                                   size_t off) {
-    copy_path(tree, log_h, idx[blockIdx.x] >> shift, out + (size_t)blockIdx.x * wpq + off);
+// the window is [row0, row0 + 2^log_h), `tree` the subtree over it
+__global__ void gather_path_kernel(const uint32_t* __restrict__ tree, size_t row0, int log_h, int shift, const uint32_t* __restrict__ idx, uint32_t* __restrict__ out,
+                                   size_t wpq, size_t off) {
+    const size_t r = (idx[blockIdx.x] >> shift) - row0;
+    if (r >> log_h) return;
+    copy_path(tree, log_h, r, out + (size_t)blockIdx.x * wpq + off);
 }
 __global__ void gather_index_kernel(const uint32_t* __restrict__ idx, uint32_t* __restrict__ out, size_t wpq) {
     if (threadIdx.x == 0) out[(size_t)blockIdx.x * wpq] = idx[blockIdx.x];
 }
-struct FriDesc { const uint32_t* fri_words; const uint32_t* fri_trees; int log_m; int n_layers; size_t word_off[32]; size_t tree_off[32]; };
+// layer i: pair rows [row0[i], row0[i] + rows[i]) (a power of two, or 0: nothing held) at word_off[i], their subtree at tree_off[i]
+struct FriDesc {
+    const uint32_t* fri_words; const uint32_t* fri_trees; int log_m; int n_layers;
+    size_t word_off[32]; size_t tree_off[32]; size_t row0[32]; size_t rows[32];
+};
 __global__ void gather_fri_kernel(FriDesc d, const uint32_t* __restrict__ idx, uint32_t* __restrict__ out, size_t wpq, size_t off) {
     const size_t r = idx[blockIdx.x];
     uint32_t* o = out + (size_t)blockIdx.x * wpq + off;
     for (int i = 0; i < d.n_layers; i++) {
-        const int log_h = d.log_m - 1 - i;
-        const size_t j = r >> (i + 1);
-        const uint32_t* row = d.fri_words + d.word_off[i] + 8 * j;
-        for (uint32_t e = threadIdx.x; e < 8; e += blockDim.x) o[e] = bb::from_monty(row[e]);
-        o += 8;
-        copy_path(d.fri_trees + d.tree_off[i], log_h, j, o);
-        o += 8 * log_h;
+        const size_t j = (r >> (i + 1)) - d.row0[i];
+        if (j < d.rows[i]) {
+            const uint32_t* row = d.fri_words + d.word_off[i] + 8 * j;
+            for (uint32_t e = threadIdx.x; e < 8; e += blockDim.x) o[e] = bb::from_monty(row[e]);
+            copy_path(d.fri_trees + d.tree_off[i], __ffsll((long long)d.rows[i]) - 1, j, o + 8);
+        }
+        o += 8 + 8 * (d.log_m - 1 - i);
     }
 }
 }  // namespace fri

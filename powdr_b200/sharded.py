@@ -135,9 +135,11 @@ class ThreadComm(Comm):
         g.barrier.wait(timeout=120)
 
 
-def prove_segment_threads(world, trace, bytecode, spans, device=0, on_device=True, fri_params=(8, 4), bus=None, want_queries=False):
+def prove_segment_threads(world, trace, bytecode, spans, device=0, on_device=True, fri_params=(8, 4), bus=None, want_queries=False,
+                          stage_ms=None):
     """Prove one segment with `world` thread-ranks on one GPU (parity harness).  trace: canonical (W, N) uint32.
-    -> list of per-rank proof dicts (all equal); with want_queries, list of (proof dict, query openings) per rank."""
+    -> list of per-rank proof dicts (all equal); with want_queries, list of (proof dict, query openings) per rank.
+    stage_ms (optional list of `world` slots): each rank's Context.last_stage_ms() after its proof."""
     from .capi import Context
     width, n = trace.shape
     log_n = n.bit_length() - 1
@@ -160,6 +162,8 @@ def prove_segment_threads(world, trace, bytecode, spans, device=0, on_device=Tru
                 host = ((host.astype(np.uint64) * np.uint64((1 << 32) % 2013265921)) % np.uint64(2013265921)).astype(np.uint32)
                 ptr = host.ctypes.data if count else 0
             out[rank] = ctx.prove_segment_sharded(air, ptr, log_n, width, comm, on_device=on_device)
+            if stage_ms is not None:
+                stage_ms[rank] = ctx.last_stage_ms()
             if want_queries:
                 out[rank] = (out[rank], ctx.query_segment_sharded(comm, log_n, width, air.perm_width))
             if comm.error:

@@ -107,6 +107,39 @@ def test_sharded_logup_segment_equals_single_gpu_and_oracle(ctx, orc, world, log
         assert p == single
 
 
+@pytest.mark.parametrize("world", [2, 4])
+@pytest.mark.parametrize("n_ints", [0, 7])
+def test_stage_clocks_of_every_prover_add_up_to_the_total(ctx, world, n_ints):
+    """pb_last_stage_ms after pb_prove_segment, pb_prove_chips and every rank of pb_prove_segment_sharded: all 12 slots are set
+    (>= 0) and the 11 stages add up to the total"""
+    from powdr_b200 import machine as M
+    from powdr_b200.sharded import prove_segment_threads
+    base = M.synthetic_machine(12, 4, seed=9)
+    mach = M.SymbolicMachine(base.constraints, M.synthetic_bus(base, n_ints, 70 + world, quadratic_every=4)) if n_ints else base
+    bc, spans = M.compile_constraints(mach)
+    bus = M.compile_bus(mach, 1) if n_ints else None
+    log_n = 10
+    trace = rand_field(np.random.default_rng(world + n_ints), (mach.width, 1 << log_n))
+    air = ctx.air(bc, spans, mach.width, bus)
+    d = ctx.to_device(trace)
+    small = M.synthetic_machine(5, 3, seed=2)
+    sbc, sspans = M.compile_constraints(small)
+    sair = ctx.air(sbc, sspans, small.width, None)
+    sd = ctx.to_device(rand_field(np.random.default_rng(1), (small.width, 1 << 7)))
+    clocks = []
+    ctx.prove_segment(air, d.ptr, log_n, mach.width, on_device=True)
+    clocks.append(("segment", ctx.last_stage_ms()))
+    ctx.prove_chips([(air, d.ptr, log_n, mach.width), (sair, sd.ptr, 7, small.width)], want_queries=False)
+    clocks.append(("chips", ctx.last_stage_ms()))
+    ranks = [None] * world
+    prove_segment_threads(world, trace, bc, spans, bus=bus, stage_ms=ranks)
+    clocks += [("sharded rank %d" % r, ms) for r, ms in enumerate(ranks)]
+    for who, ms in clocks:
+        v = list(ms.values())
+        assert len(v) == 12 and all(x >= 0 for x in v), (who, ms)
+        assert sum(v[:11]) == pytest.approx(v[11], rel=1e-5, abs=1e-3), (who, ms)
+
+
 @pytest.mark.parametrize("world,log_n,width,n_ints,small", [(2, 9, 21, 9, "14"), (4, 10, 30, 25, "3"), (8, 9, 12, 0, "2"), (4, 13, 9, 4, "6"), (2, 7, 5, 0, "24")])
 def test_sharded_query_phase_equals_single_gpu(ctx, orc, monkeypatch, world, log_n, width, n_ints, small):
     """pb_query_segment_sharded: rows and the bottom of every Merkle path from the rank that owns the row block, the top log2(world)
