@@ -151,9 +151,9 @@ int pb_prove_segment(pb_ctx_t* ctx, const pb_air_t* air, const uint32_t* trace, 
  *     when perm_width = 0) | quotient row (8) | quotient path (log_m x 8) | per FRI layer i: opened pair row (8), path ((log_m-1-i) x 8) ]
  * pb_last_openings: the opened values, [(width + 2*perm_width + 8)][4] canonical:
  *   main at zeta | perm at zeta | perm at zeta*w | quotient chunks at zeta. */
-/* ONE proof state per context: pb_prove_segment, pb_prove_segment_sharded and pb_prove_chips share workspaces, so each of them, even when
- * it fails, invalidates the query state of any earlier proof of the context; each pb_query_* answers only for a proof of its own prover,
- * pb_last_openings for pb_prove_segment and pb_prove_segment_sharded (otherwise they return PB_ERR_INVALID_ARG). */
+/* ONE proof state per context: pb_prove_segment, pb_prove_segment_sharded, pb_prove_chips and pb_prove_chips_sharded share workspaces, so
+ * each of them, even when it fails, invalidates the query state of any earlier proof of the context; each pb_query_* answers only for a
+ * proof of its own prover, pb_last_openings for pb_prove_segment and pb_prove_segment_sharded (otherwise they return PB_ERR_INVALID_ARG). */
 int pb_query_words(size_t log_n, size_t width, size_t perm_width, size_t* words_per_query);
 int pb_query_segment(pb_ctx_t* ctx, uint32_t* h_out, size_t out_capacity_words);
 int pb_last_openings(pb_ctx_t* ctx, uint32_t* h_ys, size_t capacity_words);
@@ -232,6 +232,20 @@ int pb_prove_segment_sharded(pb_ctx_t* ctx, const pb_air_t* air, const uint32_t*
  * words as pb_query_segment after pb_prove_segment on the gathered trace, on every rank.  A row and the bottom of its Merkle path come
  * from the rank that holds that row block, the top log2(world) levels from the subtree roots kept at commit time; one all-gather. */
 int pb_query_segment_sharded(pb_ctx_t* ctx, const pb_comm_t* comm, uint32_t* h_out, size_t out_capacity_words);
+/* ALL chips of a segment under one transcript across the same ranks: the proof, cumulative sums, opened values and query words of
+ * pb_prove_chips + pb_query_chips on the gathered traces, word for word, on every rank.  Every rank passes all chips in the same order;
+ * chips[c].d_trace = this rank's column block pb_shard_columns(chips[c].width, world, rank) (device, Montgomery; NULL when the block is
+ * empty), chips[c].width = the whole width.  Rank r holds rows [r*2^h/G, (r+1)*2^h/G) of the bit-reversed LDE of every chip of LDE height
+ * 2^h, so the mixed-height commitments, reduced openings and FRI injections are local to a rank (DESIGN.md §6); every exchange is one
+ * collective for all chips, so their number does not depend on n_chips.  A chip shorter than 2^(g+3) rows on G = 2^g ranks, or a world
+ * other than 2, 4, 8, 16, is PB_ERR_UNSUPPORTED.  Failure semantics as pb_prove_segment_sharded's: arguments are checked before the first
+ * collective.  pb_prove_segment_sharded is the one-chip case. */
+int pb_prove_chips_sharded(pb_ctx_t* ctx, const pb_chip_t* chips, size_t n_chips, const pb_comm_t* comm, pb_chips_proof_t* proof,
+                           uint32_t* h_cumsums);
+/* collective over the same ranks, on every rank: the queries and opened values pb_query_chips returns after pb_prove_chips on the gathered
+ * traces (layout: pb_chips_sizes); h_queries / h_ys may be NULL (no queries: no collective) */
+int pb_query_chips_sharded(pb_ctx_t* ctx, const pb_comm_t* comm, uint32_t* h_queries, size_t queries_capacity_words, uint32_t* h_ys,
+                           size_t ys_capacity_words);
 
 /* The Fiat-Shamir transcript (DuplexChallenger over Poseidon2, width 16, rate 8) runs on the HOST: absorbing the opened values is a
  * serial sponge (4363 dependent permutations for the keccak shape), so it uses an AVX-512 permutation with the whole state in one
@@ -239,7 +253,7 @@ int pb_query_segment_sharded(pb_ctx_t* ctx, const pb_comm_t* comm, uint32_t* h_o
  * times with the default constants, canonical words in and out, without a device: a known-answer / cross-check hook. */
 int pb_host_poseidon2_permute(uint32_t state[16], int reps, int force_scalar, int* used_avx512);
 
-/* per-stage device milliseconds of the last pb_prove_segment, pb_prove_chips or pb_prove_segment_sharded:
+/* per-stage device milliseconds of the last pb_prove_segment, pb_prove_chips, pb_prove_segment_sharded or pb_prove_chips_sharded:
  * [h2d, lde, merkle, logup_gen, logup_commit, quotient, qlde, qmerkle, open, fri, pow, total]; for several chips a stage spans that
  * phase of every chip (pb_prove_chips runs each phase for all chips before the next). */
 #define PB_N_STAGES 12

@@ -18,6 +18,7 @@ EXPORTS = [
     "pb_merkle_commit_rows8", "pb_poseidon2_permute", "pb_fri_fold", "pb_eval_at_point", "pb_deep_quotient", "pb_prove_segment", "pb_query_words", "pb_query_segment", "pb_last_openings", "pb_last_stage_ms",
     "pb_ctx_set_fri_params", "pb_air_set_interactions", "pb_air_perm_width", "pb_air_logup_compile_only", "pb_allgather_caps", "pb_bus_compile", "pb_bus_free", "pb_bus_apply",
     "pb_shard_columns", "pb_lde_shard", "pb_prove_segment_sharded", "pb_query_segment_sharded", "pb_prove_chips", "pb_chips_sizes", "pb_query_chips", "pb_host_poseidon2_permute",
+    "pb_prove_chips_sharded", "pb_query_chips_sharded",
     "pb_launch_count", "pb_leaf_kernel_profile", "_apc_tracegen", "_apc_apply_derived_expr", "_apc_apply_bus",
 ]
 
@@ -346,6 +347,30 @@ class Context:
         _chk(self.lib.pb_query_chips(self.h, q.ctypes.data_as(C.c_void_p) if q is not None else None, C.c_size_t(q.size if q is not None else 0),
                                      ys.ctypes.data_as(C.c_void_p), C.c_size_t(ys.size)), "pb_query_chips")
         return proof.as_dict(), cums, ys, q
+
+    def prove_chips_sharded(self, chips, comm, want_queries=True):
+        """one rank of a multi-GPU proof of all chips under one transcript (pb_prove_chips_sharded); comm: powdr_b200.sharded.Comm.
+        chips: [(Air, d_trace_ptr, log_n, width)] in the same order on every rank, d_trace_ptr = this rank's column block of the chip
+        (device, Montgomery; 0 when empty), width = the whole width.  -> the tuple of prove_chips, equal to it on every rank"""
+        K = len(chips)
+        arr = (Chip * K)(*[Chip(a.h.value, int(p or 0), int(ln), int(w)) for a, p, ln, w in chips])
+        proof = ChipsProof()
+        cums = np.zeros((K, 4), dtype=np.uint32)
+        _chk(self.lib.pb_prove_chips_sharded(self.h, arr, C.c_size_t(K), C.byref(comm.c), C.byref(proof), cums.ctypes.data_as(C.c_void_p)),
+             "pb_prove_chips_sharded")
+        ys, q = self.query_chips_sharded(comm, arr, want_queries)
+        return proof.as_dict(), cums, ys, q
+
+    def query_chips_sharded(self, comm, chip_arr, want_queries=True):
+        """opened values and query openings of the last prove_chips_sharded (collective when queries are asked for)"""
+        n_open, wpq = C.c_size_t(), C.c_size_t()
+        _chk(self.lib.pb_chips_sizes(chip_arr, C.c_size_t(len(chip_arr)), C.byref(n_open), C.byref(wpq)), "pb_chips_sizes")
+        ys = np.empty((n_open.value, 4), dtype=np.uint32)
+        q = np.empty((self.n_queries, wpq.value), dtype=np.uint32) if want_queries and self.n_queries else None
+        _chk(self.lib.pb_query_chips_sharded(self.h, C.byref(comm.c), q.ctypes.data_as(C.c_void_p) if q is not None else None,
+                                             C.c_size_t(q.size if q is not None else 0), ys.ctypes.data_as(C.c_void_p), C.c_size_t(ys.size)),
+             "pb_query_chips_sharded")
+        return ys, q
 
     def last_stage_ms(self):
         ms = (C.c_float * len(STAGES))()

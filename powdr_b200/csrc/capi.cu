@@ -145,8 +145,9 @@ struct pb_bus {
     std::vector<unsigned> grid_y;
 };
 
-// one chip of a proof (chips.inl): its matrices stay resident until the query phase.  pb_prove_segment and pb_prove_segment_sharded
-// use slot 0 (the sharded prover holds its row blocks there).
+// one chip of a proof (chips.inl): its matrices stay resident until the query phase.  pb_prove_segment uses slot 0.  The sharded provers
+// (shard_api.inl) hold their row blocks here; their `perm` is [my trace rows x the padded permutation columns | row sums | my permutation
+// columns, whole].
 struct McChip {
     size_t log_n = 0, width = 0, wp = 0, n_chunks = 0, e_main = 0, e_perm = 0, e_q = 0;
     const pb_air* air = nullptr;
@@ -154,6 +155,8 @@ struct McChip {
     DevBuf<uint32_t> lde, perm, perm_lde, qnat, qlde;
     bb::E4 cumsum = {{0u, 0u, 0u, 0u}};
 };
+
+namespace shard { struct Xfer; }        // one chip's slice of a batched exchange (shard_api.inl)
 
 struct pb_ctx {
     int device = 0;
@@ -181,8 +184,9 @@ struct pb_ctx {
     uint32_t n_queries = 100, pow_bits = 16;
     DevBuf<uint32_t> ws_fri_ch, ws_fri_log;  // device challenger state and the (root, beta) log of the FRI commit phase
     DevBuf<uint32_t> ws_sh_qall;             // every rank's share of the query openings
+    DevBuf<shard::Xfer> ws_sh_tab;           // chip table of the batched exchanges
     // The last proof, read by the query phase of the prover that made it (everything else stays resident on the device).
-    enum class Prover { segment, chips, sharded };
+    enum class Prover { segment, chips, sharded, chips_sharded };
     struct {
         bool valid = false;
         Prover by = Prover::segment;

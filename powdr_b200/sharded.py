@@ -1,4 +1,4 @@
-"""Collectives for pb_prove_segment_sharded (include/powdr_b200.h, pb_comm_t): the library takes two callbacks on DEVICE
+"""Collectives for pb_prove_segment_sharded and pb_prove_chips_sharded (include/powdr_b200.h, pb_comm_t): the library takes two callbacks on DEVICE
 pointers and links no communication library itself.
 
   TorchComm   -- one process per GPU, torch.distributed (NCCL over NVLink/NVSwitch); what bench.py uses for --gpus N > 1
@@ -105,8 +105,12 @@ class ThreadGroup:
 
 
 class ThreadComm(Comm):
+    """calls / bytes: collectives made and bytes received by this rank, per kind ("all_gather", "all_to_all")"""
+
     def __init__(self, group, rank, ctx):
         self.group, self.ctx = group, ctx
+        self.calls = {"all_gather": 0, "all_to_all": 0}
+        self.bytes = {"all_gather": 0, "all_to_all": 0}
         super().__init__(rank, group.world)
 
     def _d2h(self, ptr, nbytes):
@@ -122,6 +126,8 @@ class ThreadComm(Comm):
 
     def all_gather(self, send, recv, nbytes):
         g = self.group
+        self.calls["all_gather"] += 1
+        self.bytes["all_gather"] += nbytes * self.world
         g.slots[self.rank] = self._d2h(send, nbytes)
         g.barrier.wait(timeout=120)
         self._h2d(recv, np.concatenate(g.slots))
@@ -129,17 +135,84 @@ class ThreadComm(Comm):
 
     def all_to_all(self, send, recv, nbytes):
         g = self.group
+        self.calls["all_to_all"] += 1
+        self.bytes["all_to_all"] += nbytes * self.world
         g.slots[self.rank] = self._d2h(send, nbytes * self.world)
         g.barrier.wait(timeout=120)
         self._h2d(recv, np.concatenate([g.slots[r][self.rank * nbytes:(self.rank + 1) * nbytes] for r in range(self.world)]))
         g.barrier.wait(timeout=120)
 
 
+def _run_ranks(world, body):
+    """body(rank, group) on `world` threads; the first real error is raised (a broken barrier only follows another rank's error)"""
+    group = ThreadGroup(world)
+    out, errs = [None] * world, [None] * world
+
+    def run(rank):
+        try:
+            out[rank] = body(rank, group)
+        except BaseException as e:      # noqa: BLE001
+            errs[rank] = e
+            group.barrier.abort()
+
+    threads = [threading.Thread(target=run, args=(r,)) for r in range(world)]
+    for t in threads:
+        t.start()
+    for t in threads:
+        t.join()
+    for e in errs:
+        if e is not None and not isinstance(e, threading.BrokenBarrierError):
+            raise e
+    for e in errs:
+        if e is not None:
+            raise e
+    return out
+
+
+def prove_chips_threads(world, chips, device=0, fri_params=(8, 4), want_queries=True, stats=None, comm_factory=None):
+    """Prove all chips of a segment under one transcript with `world` thread-ranks on one GPU (pb_prove_chips_sharded).  chips:
+    [(trace canonical (W, N) uint32, bytecode, spans, bus or None)]; each rank compiles its own AIRs and passes its column block of
+    every chip.  -> per rank the tuple of Context.prove_chips (proof dict, cumulative sums, opened values, queries or None).
+    stats (optional list of `world` slots): per rank {"calls", "bytes", "launches", "stage_ms"} of the proof and query phase.
+    comm_factory(group, rank, ctx) (optional) makes the rank's Comm instead of a ThreadComm."""
+    from .capi import Context
+
+    def body(rank, group):
+        ctx = Context(device)
+        try:
+            ctx.set_fri_params(*fri_params)
+            airs, bufs, args = [], [], []
+            for trace, bc, spans, bus in chips:
+                width, n = trace.shape
+                air = ctx.air(bc, spans, width, bus)
+                first, count = shard_columns(width, world, rank)
+                buf = ctx.to_device(trace[first:first + count]) if count else None
+                airs.append(air)
+                bufs.append(buf)
+                args.append((air, buf.ptr if buf else 0, n.bit_length() - 1, width))
+            comm = comm_factory(group, rank, ctx) if comm_factory else ThreadComm(group, rank, ctx)
+            l0 = ctx.launch_count()
+            res = ctx.prove_chips_sharded(args, comm, want_queries=want_queries)
+            if comm.error:
+                raise comm.error
+            if stats is not None:
+                stats[rank] = {"calls": dict(getattr(comm, "calls", {})), "bytes": dict(getattr(comm, "bytes", {})),
+                               "launches": ctx.launch_count() - l0, "stage_ms": ctx.last_stage_ms()}
+            for a in airs:
+                a.free()
+            return res
+        finally:
+            ctx.close()
+
+    return _run_ranks(world, body)
+
+
 def prove_segment_threads(world, trace, bytecode, spans, device=0, on_device=True, fri_params=(8, 4), bus=None, want_queries=False,
-                          stage_ms=None):
+                          stage_ms=None, stats=None):
     """Prove one segment with `world` thread-ranks on one GPU (parity harness).  trace: canonical (W, N) uint32.
     -> list of per-rank proof dicts (all equal); with want_queries, list of (proof dict, query openings) per rank.
-    stage_ms (optional list of `world` slots): each rank's Context.last_stage_ms() after its proof."""
+    stage_ms (optional list of `world` slots): each rank's Context.last_stage_ms() after its proof.
+    stats (optional list of `world` slots): each rank's collective calls and bytes (ThreadComm.calls / .bytes) and kernel launches."""
     from .capi import Context
     width, n = trace.shape
     log_n = n.bit_length() - 1
@@ -161,11 +234,14 @@ def prove_segment_threads(world, trace, bytecode, spans, device=0, on_device=Tru
                 host = np.ascontiguousarray(trace[first:first + count])
                 host = ((host.astype(np.uint64) * np.uint64((1 << 32) % 2013265921)) % np.uint64(2013265921)).astype(np.uint32)
                 ptr = host.ctypes.data if count else 0
+            l0 = ctx.launch_count()
             out[rank] = ctx.prove_segment_sharded(air, ptr, log_n, width, comm, on_device=on_device)
             if stage_ms is not None:
                 stage_ms[rank] = ctx.last_stage_ms()
             if want_queries:
                 out[rank] = (out[rank], ctx.query_segment_sharded(comm, log_n, width, air.perm_width))
+            if stats is not None:
+                stats[rank] = {"calls": dict(comm.calls), "bytes": dict(comm.bytes), "launches": ctx.launch_count() - l0}
             if comm.error:
                 raise comm.error
         except BaseException as e:      # noqa: BLE001
