@@ -156,6 +156,8 @@ struct McChip {
     bb::E4 cumsum = {{0u, 0u, 0u, 0u}};
 };
 
+struct Mat { const uint32_t* p; size_t width; size_t log_h; };      // a committed matrix, column-major [width][2^log_h]
+
 namespace shard { struct Xfer; }        // one chip's slice of a batched exchange (shard_api.inl)
 
 struct pb_ctx {

@@ -473,14 +473,20 @@ __global__ void __launch_bounds__(256) scan_add_kernel(uint32_t* __restrict__ ou
 // the three phi constraints, then the division by Z_H and the chunk split (the tail of the quotient when the AIR has interactions).
 //   acc = raw + alpha^2 * is_first * (phi - S) + alpha * is_trans * (phi' - phi - S') + is_last * (phi - cumsum)
 // rows are LDE rows in bit-reversed order; ' = the LDE point 2 steps on in natural order (the next trace row).
-__global__ void __launch_bounds__(256) finish_kernel(const uint32_t* __restrict__ raw, const uint32_t* __restrict__ ssum, const uint32_t* __restrict__ phi /* [4][m] */,
-                                                     size_t m, int log_n, uint32_t shift_m, uint32_t omega_m_m, uint32_t w_n_inv_m, uint32_t sn_m,
-                                                     bb::E4 alpha, bb::E4 alpha2, bb::E4 cumsum, uint32_t zinv0, uint32_t zinv1, uint32_t* __restrict__ out) {
-    const size_t r = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+// The kernel does rows [row0, row0 + 2^log_ms) of the 2N: raw is [4][2^log_ms] over them.  ssum and phi are given as row blocks of
+// 2^log_ms rows, block b's [4][2^log_ms] at b * blk_stride, because the next row may lie in another block (the whole matrix: one block,
+// log_ms = log_n + 1).  out: the quotient of these rows split at the coset boundary, [rows / N][4][min(rows, N)].
+__global__ void __launch_bounds__(256) finish_kernel(const uint32_t* __restrict__ raw, const uint32_t* __restrict__ ssum, const uint32_t* __restrict__ phi,
+                                                     size_t blk_stride, int log_ms, size_t row0, int log_n, uint32_t shift_m, uint32_t omega_m_m,
+                                                     uint32_t w_n_inv_m, uint32_t sn_m, bb::E4 alpha, bb::E4 alpha2, bb::E4 cumsum, uint32_t zinv0,
+                                                     uint32_t zinv1, uint32_t* __restrict__ out) {
+    const size_t r = (size_t)blockIdx.x * blockDim.x + threadIdx.x, m = (size_t)1 << log_ms;
     if (r >= m) return;
     const int log_m = log_n + 1;
-    const uint32_t i_nat = __brev((uint32_t)r) >> (32 - log_m);
-    const size_t rn = __brev((uint32_t)((i_nat + 2) & (uint32_t)(m - 1))) >> (32 - log_m);
+    const size_t R = row0 + r;
+    const uint32_t i_nat = __brev((uint32_t)R) >> (32 - log_m);
+    const size_t Rn = __brev((i_nat + 2) & (uint32_t)(((size_t)1 << log_m) - 1)) >> (32 - log_m);
+    const size_t here = (R >> log_ms) * blk_stride + r, next = (Rn >> log_ms) * blk_stride + (Rn & (m - 1));
     const uint32_t x = bb::mul(shift_m, bb::pow(omega_m_m, (uint64_t)i_nat));
     const uint32_t zh = bb::sub((i_nat & 1) ? bb::neg(sn_m) : sn_m, bb::R1);
     const uint32_t is_first = bb::mul(zh, bb::inv(bb::sub(x, bb::R1)));
@@ -490,18 +496,19 @@ __global__ void __launch_bounds__(256) finish_kernel(const uint32_t* __restrict_
 #pragma unroll
     for (int l = 0; l < 4; l++) {
         acc.c[l] = raw[(size_t)l * m + r];
-        S.c[l] = ssum[(size_t)l * m + r];
-        Sn.c[l] = ssum[(size_t)l * m + rn];
-        ph.c[l] = phi[(size_t)l * m + r];
-        phn.c[l] = phi[(size_t)l * m + rn];
+        S.c[l] = ssum[(size_t)l * m + here];
+        Sn.c[l] = ssum[(size_t)l * m + next];
+        ph.c[l] = phi[(size_t)l * m + here];
+        phn.c[l] = phi[(size_t)l * m + next];
     }
     acc = bb::e4_add(acc, bb::e4_mul(alpha2, bb::e4_scale(bb::e4_sub(ph, S), is_first)));
     acc = bb::e4_add(acc, bb::e4_mul(alpha, bb::e4_scale(bb::e4_sub(bb::e4_sub(phn, ph), Sn), is_trans)));
     acc = bb::e4_add(acc, bb::e4_scale(bb::e4_sub(ph, cumsum), is_last));
-    const size_t n = (size_t)1 << log_n, chunk = r >> log_n, j = r & (n - 1);
-    const uint32_t z = chunk ? zinv1 : zinv0;
+    const int log_ld = min(log_ms, log_n);
+    const size_t ld = (size_t)1 << log_ld, chunk = r >> log_ld, j = r & (ld - 1);
+    const uint32_t z = (R >> log_n) ? zinv1 : zinv0;
 #pragma unroll
-    for (int l = 0; l < 4; l++) out[(chunk * 4 + l) * n + j] = bb::mul(acc.c[l], z);
+    for (int l = 0; l < 4; l++) out[(chunk * 4 + l) * ld + j] = bb::mul(acc.c[l], z);
 }
 
 }  // namespace logup

@@ -216,13 +216,10 @@ def prove_segment_threads(world, trace, bytecode, spans, device=0, on_device=Tru
     from .capi import Context
     width, n = trace.shape
     log_n = n.bit_length() - 1
-    group = ThreadGroup(world)
-    out, errs = [None] * world, [None] * world
 
-    def run(rank):
-        ctx = None
+    def body(rank, group):
+        ctx = Context(device)
         try:
-            ctx = Context(device)
             ctx.set_fri_params(*fri_params)
             air = ctx.air(bytecode, spans, width, bus)
             first, count = shard_columns(width, world, rank)
@@ -235,31 +232,17 @@ def prove_segment_threads(world, trace, bytecode, spans, device=0, on_device=Tru
                 host = ((host.astype(np.uint64) * np.uint64((1 << 32) % 2013265921)) % np.uint64(2013265921)).astype(np.uint32)
                 ptr = host.ctypes.data if count else 0
             l0 = ctx.launch_count()
-            out[rank] = ctx.prove_segment_sharded(air, ptr, log_n, width, comm, on_device=on_device)
+            res = ctx.prove_segment_sharded(air, ptr, log_n, width, comm, on_device=on_device)
             if stage_ms is not None:
                 stage_ms[rank] = ctx.last_stage_ms()
             if want_queries:
-                out[rank] = (out[rank], ctx.query_segment_sharded(comm, log_n, width, air.perm_width))
+                res = (res, ctx.query_segment_sharded(comm, log_n, width, air.perm_width))
             if stats is not None:
                 stats[rank] = {"calls": dict(comm.calls), "bytes": dict(comm.bytes), "launches": ctx.launch_count() - l0}
             if comm.error:
                 raise comm.error
-        except BaseException as e:      # noqa: BLE001
-            errs[rank] = e
-            group.barrier.abort()
+            return res
         finally:
-            if ctx is not None:
-                ctx.close()
+            ctx.close()
 
-    threads = [threading.Thread(target=run, args=(r,)) for r in range(world)]
-    for t in threads:
-        t.start()
-    for t in threads:
-        t.join()
-    for e in errs:
-        if e is not None and not isinstance(e, threading.BrokenBarrierError):
-            raise e
-    for e in errs:
-        if e is not None:
-            raise e
-    return out
+    return _run_ranks(world, body)
