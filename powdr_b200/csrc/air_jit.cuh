@@ -304,8 +304,7 @@ inline int build(const std::vector<uint32_t>& code, const std::vector<air::Span>
     if (code.size() > 1000000) return 2;                       // keep compile time bounded; huge AIRs stay on the interpreter
     Api& a = api();
     if (!a.nvrtc_ok || (out && !a.ok)) return 3;
-    size_t chunk_words = 2000;      // keccak shape (7.2 k words): 4 modules, 2.7 s instead of 7.8 s; sha256 shape: 13 s; 141 k-word pre-opt machine: 30 s
-    if (const char* e = getenv("PB_AIR_JIT_CHUNK")) chunk_words = std::max<size_t>(100, (size_t)atol(e));
+    const size_t chunk_words = 2000;      // keccak shape (7.2 k words): 4 modules, 2.7 s instead of 7.8 s; sha256 shape: 13 s; 141 k-word pre-opt machine: 30 s
     std::vector<size_t> bounds{0};
     for (size_t k = 0, w = 0; k < spans.size(); k++) {
         if (w > 0 && w + spans[k].len > chunk_words) { bounds.push_back(k); w = 0; }
@@ -327,8 +326,7 @@ inline int build(const std::vector<uint32_t>& code, const std::vector<air::Span>
             }
         }
     };
-    size_t n_threads = std::min<size_t>(n_chunks, std::max(1u, std::thread::hardware_concurrency()));
-    if (const char* e = getenv("PB_AIR_JIT_THREADS")) n_threads = std::min<size_t>(n_chunks, std::max<size_t>(1, (size_t)atol(e)));
+    const size_t n_threads = std::min<size_t>(n_chunks, std::max(1u, std::thread::hardware_concurrency()));
     std::vector<std::thread> pool_threads;
     for (size_t t = 1; t < n_threads; t++) pool_threads.emplace_back(worker);
     worker();

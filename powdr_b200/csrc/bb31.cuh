@@ -30,13 +30,6 @@ BB_HD uint32_t sub(uint32_t a, uint32_t b) {
     uint32_t d = a - b, e = d + P;
     return e < d ? e : d;                   // a>=b: d<p<=e (no wrap) -> d ; a<b: d wraps high, e = d+P wraps low -> e
 }
-__device__ __forceinline__ uint32_t add_lin(uint32_t a, uint32_t b) {   // add used by the Poseidon2 external layer
-#ifdef PB_V_LIN_PIN
-    return reduce_2p(__viaddmin_u32(a, b, 0xffffffffu));
-#else
-    return reduce_2p(a + b);
-#endif
-}
 BB_HD uint32_t neg(uint32_t a) { return a ? P - a : 0u; }
 BB_HD uint32_t dbl(uint32_t a) { return reduce_2p(a + a); }
 
@@ -57,18 +50,8 @@ BB_HD int32_t smul(int32_t a, int32_t b) {
     int32_t lo, hi;
     asm("mul.wide.s32 %0, %1, %2;" : "=l"(t) : "r"(a), "r"(b));
     asm("mov.b64 {%0, %1}, %2;" : "=r"(lo), "=r"(hi) : "l"(t));
-#ifdef PB_V_PINV_SHIFT
-    // experiment: p^-1 mod 2^32 = 2^31 + 2^27 + 1, so lo * p^-1 is two shift-adds on the ALU pipe instead of an IMAD
-    const uint32_t ulo = (uint32_t)lo;
-    int32_t m = (int32_t)(ulo + (ulo << 27) + (ulo << 31));
-#else
     int32_t m = (int32_t)((uint32_t)lo * PINV);
-#endif
-#ifdef PB_V_SMUL_PIN
-    return __viaddmin_s32(hi, -__mulhi(m, (int32_t)P), 0x7fffffff);   // experiment: pin the subtraction to the ALU pipe
-#else
     return hi - __mulhi(m, (int32_t)P);
-#endif
 #else
     int64_t t = (int64_t)a * (int64_t)b;
     int32_t m = (int32_t)((uint32_t)t * PINV);

@@ -205,8 +205,6 @@ struct pb_ctx {
         uint32_t top_main[31][8], top_perm[31][8], top_q[31][8], top_fri[32][31][8];
     } last;
     cudaStream_t copy_stream = nullptr;   // H2D chunks of the host-input pipeline
-    cudaStream_t lde_streams[8] = {nullptr};   // PB_LDE_STREAMS experiment
-    cudaEvent_t lde_join[8] = {nullptr}, lde_fork = nullptr;
     cudaEvent_t ev_copy[2] = {nullptr}, ev_free[2] = {nullptr};
     cudaEvent_t ev[12] = {nullptr};         // stage boundaries of pb_last_stage_ms (stage_clocks)
     float stage_ms[PB_N_STAGES] = {0};     // h2d, lde, merkle, logup_gen, logup_commit, quotient, qlde, qmerkle, open(+deep), fri, pow, total
@@ -376,7 +374,7 @@ int leaf_hash_cols(pb_ctx* ctx, const std::vector<const uint32_t*>& cols, size_t
 // Column batch: 16 tiles of 2^LDE_BATCH_LOG_TILE elements per SM (66 columns at 2^20 on 132 SMs).  On the H100 the passes run
 // at 40-75 % of HBM bandwidth and 3-6 butterflies/clk/SM (scripts/lde_kernels.py); batches of 2-16 columns, alone or round-robin
 // over 2-8 streams so that the K1->K2->K3 intermediates of the batches in flight fit the 50 MB L2, measured no faster at 2022 or
-// 3348 columns (scripts/lde_sweep.py, DESIGN.md §4).  PB_LDE_BATCH / PB_LDE_STREAMS override for experiments.
+// 3348 columns (DESIGN.md §4).  PB_LDE_BATCH overrides the batch size.
 constexpr int LDE_BATCH_LOG_TILE = 15;
 size_t lde_column_batch(const pb_ctx* ctx, size_t N, size_t width) {
     const size_t tiles_per_col = std::max<size_t>(1, N >> LDE_BATCH_LOG_TILE);
@@ -508,8 +506,6 @@ int pb_ctx_destroy(pb_ctx_t* ctx) {
     for (auto& t : ctx->tws) { cudaFree(t.d_inv); cudaFree(t.d_fwd); }
     if (ctx->d_fold_tab) cudaFree(ctx->d_fold_tab);
     if (ctx->copy_stream) cudaStreamDestroy(ctx->copy_stream);
-    for (int i = 0; i < 8; i++) { if (ctx->lde_streams[i]) cudaStreamDestroy(ctx->lde_streams[i]); if (ctx->lde_join[i]) cudaEventDestroy(ctx->lde_join[i]); }
-    if (ctx->lde_fork) cudaEventDestroy(ctx->lde_fork);
     for (int i = 0; i < 2; i++) { if (ctx->ev_copy[i]) cudaEventDestroy(ctx->ev_copy[i]); if (ctx->ev_free[i]) cudaEventDestroy(ctx->ev_free[i]); }
     for (auto& e : ctx->ev) if (e) cudaEventDestroy(e);
     for (int i = 0; i < pb_ctx::KPROF; i++) { if (ctx->kp_a[i]) cudaEventDestroy(ctx->kp_a[i]); if (ctx->kp_b[i]) cudaEventDestroy(ctx->kp_b[i]); }
@@ -589,39 +585,13 @@ int pb_lde_batch(pb_ctx_t* ctx, const uint32_t* d_trace, size_t log_n, size_t wi
     int rc = get_twiddles(ctx, n, (int)log_blowup, shift, &tw);
     if (rc) return rc;
     const size_t batch = lde_column_batch(ctx, N, width);
-    // PB_LDE_STREAMS > 1 (experiment): small column batches round-robin over several streams, so the four passes of different
-    // batches overlap and the intermediates of the batches in flight can stay in L2
-    int n_streams = 1;
-    if (const char* e = getenv("PB_LDE_STREAMS")) n_streams = std::min(8, std::max(1, atoi(e)));
-    rc = ctx->tmp.ensure((size_t)n_streams * batch * N); if (rc) return rc;
-    rc = ctx->tmp2.ensure((size_t)n_streams * batch * N * cosets); if (rc) return rc;
-    cudaStream_t main_stream = ctx->stream;
-    if (n_streams > 1) {
-        for (int i = 0; i < n_streams; i++)
-            if (!ctx->lde_streams[i]) {
-                CK(cudaStreamCreateWithFlags(&ctx->lde_streams[i], cudaStreamNonBlocking));
-                CK(cudaEventCreateWithFlags(&ctx->lde_join[i], cudaEventDisableTiming));
-            }
-        if (!ctx->lde_fork) CK(cudaEventCreateWithFlags(&ctx->lde_fork, cudaEventDisableTiming));
-        CK(cudaEventRecord(ctx->lde_fork, main_stream));
-        for (int i = 0; i < n_streams; i++) CK(cudaStreamWaitEvent(ctx->lde_streams[i], ctx->lde_fork, 0));
-    }
-    size_t k = 0;
-    for (size_t c0 = 0; c0 < width; c0 += batch, k++) {
+    rc = ctx->tmp.ensure(batch * N); if (rc) return rc;
+    rc = ctx->tmp2.ensure(batch * N * cosets); if (rc) return rc;
+    for (size_t c0 = 0; c0 < width; c0 += batch) {
         const unsigned nb = (unsigned)std::min(batch, width - c0);
-        const size_t sidx = k % (size_t)n_streams;
-        if (n_streams > 1) ctx->stream = ctx->lde_streams[sidx];
-        uint32_t* t1 = ctx->tmp.p + sidx * batch * N;
-        uint32_t* t2 = ctx->tmp2.p + sidx * batch * N * cosets;
-        ntt_inverse_cols(ctx, n, tw, d_trace + c0 * N, nb, t1);
-        ntt_forward_cols(ctx, n, tw, (int)log_blowup, t1, nb, t2, d_lde + c0 * N * cosets, N * cosets);
+        ntt_inverse_cols(ctx, n, tw, d_trace + c0 * N, nb, ctx->tmp.p);
+        ntt_forward_cols(ctx, n, tw, (int)log_blowup, ctx->tmp.p, nb, ctx->tmp2.p, d_lde + c0 * N * cosets, N * cosets);
     }
-    ctx->stream = main_stream;
-    if (n_streams > 1)
-        for (int i = 0; i < n_streams; i++) {
-            CK(cudaEventRecord(ctx->lde_join[i], ctx->lde_streams[i]));
-            CK(cudaStreamWaitEvent(main_stream, ctx->lde_join[i], 0));
-        }
     CK(cudaGetLastError());
     return 0;
 }

@@ -179,17 +179,10 @@ inline Val emit_expr(std::string& src, const std::vector<uint32_t>& code, air::S
     return st.back();
 }
 
-constexpr size_t GROUP_CHUNKS_MAX = 8;
-// tuning knobs of the generated kernels (experiments: PB_LOGUP_GROUP / PB_LOGUP_BLOCK / PB_LOGUP_MINB)
 // chunks per generated function: permutation kernel 2 (one inversion per 2 chunks), fold kernel 1 -- fewer live Ext4 values beat
 // the amortised inversion
-inline size_t group_chunks(bool for_perm) {
-    if (const char* e = getenv(for_perm ? "PB_LOGUP_GROUP_PERM" : "PB_LOGUP_GROUP_FOLD")) return std::min<size_t>(GROUP_CHUNKS_MAX, std::max<size_t>(1, (size_t)atol(e)));
-    if (const char* e = getenv("PB_LOGUP_GROUP")) return std::min<size_t>(GROUP_CHUNKS_MAX, std::max<size_t>(1, (size_t)atol(e)));
-    return for_perm ? 2 : 1;
-}
-inline unsigned block_threads() { if (const char* e = getenv("PB_LOGUP_BLOCK")) return (unsigned)std::min(1024l, std::max(32l, atol(e))); return 128; }
-inline unsigned min_blocks() { if (const char* e = getenv("PB_LOGUP_MINB")) return (unsigned)std::max(0l, atol(e)); return 0; }
+constexpr size_t PERM_GROUP_CHUNKS = 2, FOLD_GROUP_CHUNKS = 1;
+constexpr unsigned BLOCK_THREADS = 128;     // threads per CTA of both generated kernels
 
 // source of one module covering chunks [c_begin, c_end): both kernels.  lits_out: literal arguments found (recorded once per interaction).
 inline std::string generate(const std::vector<uint32_t>& code, const std::vector<air::Span>& spans, const std::vector<uint32_t>& pool, const Program& p,
@@ -198,12 +191,11 @@ inline std::string generate(const std::vector<uint32_t>& code, const std::vector
     src += LU_PRELUDE;
     char buf[512];
     std::string perm_calls, fold_calls;
-    const unsigned BT = block_threads(), MINB = min_blocks();
     // one __noinline__ function per group of chunks; the two kernels use their own group size (the permutation kernel amortises one
     // Ext4 inversion over the group, the fold kernel has nothing to share between chunks and runs best with the fewest live values)
     for (int kind = 0; kind < 2; kind++) {
         const bool for_perm = kind == 0;
-        const size_t GROUP = group_chunks(for_perm);
+        const size_t GROUP = for_perm ? PERM_GROUP_CHUNKS : FOLD_GROUP_CHUNKS;
         size_t n_groups = 0;
         for (size_t cb = c_begin; cb < c_end; cb += GROUP, n_groups++) {
             const size_t ce = std::min(c_end, cb + GROUP);
@@ -312,7 +304,7 @@ inline std::string generate(const std::vector<uint32_t>& code, const std::vector
         }
     }
     char lb[64];
-    if (MINB) snprintf(lb, sizeof lb, "__launch_bounds__(%u, %u)", BT, MINB); else snprintf(lb, sizeof lb, "__launch_bounds__(%u)", BT);
+    snprintf(lb, sizeof lb, "__launch_bounds__(%u)", BLOCK_THREADS);
     src += std::string("\nextern \"C\" __global__ void ") + lb + R"( pbl_perm(const u32* __restrict__ mat, u64 n, const uint4* __restrict__ kc, const uint4* __restrict__ bt,
                                                             u32* __restrict__ perm, u32* __restrict__ rowsum, int first) {
     const u64 r = (u64)blockIdx.x * blockDim.x + threadIdx.x;
@@ -352,8 +344,7 @@ inline int build(const std::vector<uint32_t>& code, const std::vector<air::Span>
     if (!a.nvrtc_ok || (out && !a.ok)) return 3;
     // chunks per module = per kernel launch: the generated code is straight-line, every warp streams through all of it once, so a
     // module must fit the instruction cache (ncu: `no_instruction` was the top stall with 64-chunk modules = 460 KB of SASS)
-    size_t mod_chunks = 16;
-    if (const char* e = getenv("PB_LOGUP_JIT_CHUNKS")) mod_chunks = std::max<size_t>(1, (size_t)atol(e));
+    const size_t mod_chunks = 16;
     const size_t nc = p.n_chunks(), n_mods = (nc + mod_chunks - 1) / mod_chunks;
     std::vector<std::vector<char>> cubins(n_mods);
     std::vector<std::vector<LitArg>> lits(n_mods);
@@ -370,8 +361,7 @@ inline int build(const std::vector<uint32_t>& code, const std::vector<air::Span>
             }
         }
     };
-    size_t n_threads = std::min<size_t>(n_mods, std::max(1u, std::thread::hardware_concurrency()));
-    if (const char* e = getenv("PB_AIR_JIT_THREADS")) n_threads = std::min<size_t>(n_mods, std::max<size_t>(1, (size_t)atol(e)));
+    const size_t n_threads = std::min<size_t>(n_mods, std::max(1u, std::thread::hardware_concurrency()));
     std::vector<std::thread> ths;
     for (size_t t = 1; t < n_threads; t++) ths.emplace_back(worker);
     worker();
@@ -412,8 +402,8 @@ inline int launch_perm(const Kernels& k, cudaStream_t st, const uint32_t* mat, u
     for (size_t c = 0; c < k.perm_fns.size(); c++) {
         int first = c == 0;
         void* args[] = {(void*)&mat, (void*)&n, (void*)&kc, (void*)&bt, (void*)&perm, (void*)&rowsum, (void*)&first};
-        const unsigned bt = block_threads();
-        CUresult rc = airjit::api().LaunchKernel(k.perm_fns[c], (unsigned)((n + bt - 1) / bt), 1, 1, bt, 1, 1, 0, (CUstream)st, args, nullptr);
+        CUresult rc = airjit::api().LaunchKernel(k.perm_fns[c], (unsigned)((n + BLOCK_THREADS - 1) / BLOCK_THREADS), 1, 1, BLOCK_THREADS, 1, 1, 0,
+                                                 (CUstream)st, args, nullptr);
         if (rc != CUDA_SUCCESS) return 700 + (int)rc;
     }
     return 0;
@@ -423,8 +413,8 @@ inline int launch_fold(const Kernels& k, cudaStream_t st, const uint32_t* lde, c
     for (size_t c = 0; c < k.fold_fns.size(); c++) {
         int first = c == 0;
         void* args[] = {(void*)&lde, (void*)&plde, (void*)&m, (void*)&kc, (void*)&bt, (void*)&apl, (void*)&raw, (void*)&ssum, (void*)&first};
-        const unsigned bt = block_threads();
-        CUresult rc = airjit::api().LaunchKernel(k.fold_fns[c], (unsigned)((m + bt - 1) / bt), 1, 1, bt, 1, 1, 0, (CUstream)st, args, nullptr);
+        CUresult rc = airjit::api().LaunchKernel(k.fold_fns[c], (unsigned)((m + BLOCK_THREADS - 1) / BLOCK_THREADS), 1, 1, BLOCK_THREADS, 1, 1, 0,
+                                                 (CUstream)st, args, nullptr);
         if (rc != CUDA_SUCCESS) return 700 + (int)rc;
     }
     return 0;

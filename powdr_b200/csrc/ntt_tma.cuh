@@ -5,7 +5,7 @@
 // Why these passes: a K2 tile is 16 consecutive blocks of 2^10 positions of one column = ONE contiguous 64 KB span of global
 // memory, so the whole tile moves with two `cp.async.bulk.tensor.2d` boxes (32 words x 256 rows each) in and two out; no thread
 // computes a global address, issues an LDG/STG or runs a transpose loop (the per-thread tile movement and swizzled staging of
-// the LDG/STS version were 25-30 % of these kernels' instructions, profiles/README.md).
+// the LDG/STS version were 25-30 % of these kernels' instructions).
 //
 // Layout: the tensor map views the buffer as rows of 32 words (128 B) with CU_TENSOR_MAP_SWIZZLE_128B, i.e. the 16-byte chunk index
 // of a word is XORed with (row mod 8) on the way into shared memory (and back on the way out).  Block-local position t (10 bits)

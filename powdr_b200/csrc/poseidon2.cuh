@@ -22,11 +22,7 @@ struct Consts {
 __constant__ Consts c_p2;
 
 __device__ __forceinline__ uint32_t sbox_rc(uint32_t s, uint32_t rc_minus_p) {
-#ifdef PB_V_RC_PIN
-    int32_t x = __viaddmin_s32((int32_t)s, (int32_t)rc_minus_p, 0x7fffffff);
-#else
     int32_t x = (int32_t)(s + rc_minus_p);          // [-p, p)
-#endif
     int32_t x2 = bb::smul(x, x);
     int32_t x3 = bb::smul(x2, x);
     int32_t x4 = bb::smul(x2, x2);
@@ -38,24 +34,24 @@ __device__ __forceinline__ void external_linear(uint32_t (&s)[16]) {
 #pragma unroll
     for (int c = 0; c < 16; c += 4) {
         uint32_t x0 = s[c], x1 = s[c + 1], x2 = s[c + 2], x3 = s[c + 3];
-        uint32_t t01 = bb::add_lin(x0, x1), t23 = bb::add_lin(x2, x3);
-        uint32_t t0123 = bb::add_lin(t01, t23);
-        uint32_t t01123 = bb::add_lin(t0123, x1), t01233 = bb::add_lin(t0123, x3);
-        s[c + 3] = bb::add_lin(t01233, bb::add_lin(x0, x0));
-        s[c + 1] = bb::add_lin(t01123, bb::add_lin(x2, x2));
-        s[c] = bb::add_lin(t01123, t01);
-        s[c + 2] = bb::add_lin(t01233, t23);
+        uint32_t t01 = bb::add(x0, x1), t23 = bb::add(x2, x3);
+        uint32_t t0123 = bb::add(t01, t23);
+        uint32_t t01123 = bb::add(t0123, x1), t01233 = bb::add(t0123, x3);
+        s[c + 3] = bb::add(t01233, bb::add(x0, x0));
+        s[c + 1] = bb::add(t01123, bb::add(x2, x2));
+        s[c] = bb::add(t01123, t01);
+        s[c + 2] = bb::add(t01233, t23);
     }
-    uint32_t q0 = bb::add_lin(bb::add_lin(s[0], s[4]), bb::add_lin(s[8], s[12]));
-    uint32_t q1 = bb::add_lin(bb::add_lin(s[1], s[5]), bb::add_lin(s[9], s[13]));
-    uint32_t q2 = bb::add_lin(bb::add_lin(s[2], s[6]), bb::add_lin(s[10], s[14]));
-    uint32_t q3 = bb::add_lin(bb::add_lin(s[3], s[7]), bb::add_lin(s[11], s[15]));
+    uint32_t q0 = bb::add(bb::add(s[0], s[4]), bb::add(s[8], s[12]));
+    uint32_t q1 = bb::add(bb::add(s[1], s[5]), bb::add(s[9], s[13]));
+    uint32_t q2 = bb::add(bb::add(s[2], s[6]), bb::add(s[10], s[14]));
+    uint32_t q3 = bb::add(bb::add(s[3], s[7]), bb::add(s[11], s[15]));
 #pragma unroll
     for (int c = 0; c < 16; c += 4) {
-        s[c] = bb::add_lin(s[c], q0);
-        s[c + 1] = bb::add_lin(s[c + 1], q1);
-        s[c + 2] = bb::add_lin(s[c + 2], q2);
-        s[c + 3] = bb::add_lin(s[c + 3], q3);
+        s[c] = bb::add(s[c], q0);
+        s[c + 1] = bb::add(s[c + 1], q1);
+        s[c + 2] = bb::add(s[c + 2], q2);
+        s[c + 3] = bb::add(s[c + 3], q3);
     }
 }
 
@@ -82,7 +78,6 @@ __device__ __forceinline__ void internal_round(uint32_t (&s)[16], int r) {
     uint32_t c = bb::add(bb::add(s[8], s[9]), bb::add(s[10], s[11]));
     uint32_t d = bb::add(bb::add(s[12], s[13]), bb::add(s[14], s[15]));
     uint32_t sum = bb::add(bb::add(a, b), bb::add(c, d));
-#ifndef PB_V_DIAG_SHOUP      // default since round 2: +2 % leaf-hashing rate (profiles/README.md); -DPB_V_DIAG_SHOUP restores the Shoup products
     if (c_p2.p3_diag) {
         // every entry of the Plonky3 diagonal [-2,1,2,1/2,3,4,-1/2,-3,-4,2^-8,1/4,1/8,2^-27,-2^-8,-1/16,-2^-27] without a modular
         // product: small multiples as add chains, the 2^-K entries through div_2k -- the multiplier pipe is the binding one
@@ -103,22 +98,7 @@ __device__ __forceinline__ void internal_round(uint32_t (&s)[16], int r) {
         s[13] = bb::sub(sum, div_2k<8>(s[13]));            // -2^-8
         s[14] = bb::sub(sum, div_2k<4>(s[14]));            // -1/16
         s[15] = bb::sub(sum, div_2k<27>(s[15]));           // -2^-27
-    } else
-#else
-    if (c_p2.p3_diag) {
-        // the cheap entries of the Plonky3 diagonal go to the ALU pipe (which has slack), the rest to Shoup products
-        s[0] = bb::sub(bb::sub(sum, s[0]), s[0]);          // -2
-        s[1] = bb::add(sum, s[1]);                         //  1
-        s[2] = bb::add(sum, bb::dbl(s[2]));                //  2
-        s[3] = bb::add(sum, halve(s[3]));                  //  1/2
-        s[6] = bb::sub(sum, halve(s[6]));                  // -1/2
-        s[4] = bb::add(sum, mul_const(s[4], c_p2.diag_w[4], c_p2.diag_wp[4]));
-        s[5] = bb::add(sum, mul_const(s[5], c_p2.diag_w[5], c_p2.diag_wp[5]));
-#pragma unroll
-        for (int i = 7; i < 16; i++) s[i] = bb::add(sum, mul_const(s[i], c_p2.diag_w[i], c_p2.diag_wp[i]));
-    } else
-#endif
-    {
+    } else {
 #pragma unroll
         for (int i = 0; i < 16; i++) s[i] = bb::add(sum, mul_const(s[i], c_p2.diag_w[i], c_p2.diag_wp[i]));
     }
@@ -152,24 +132,14 @@ constexpr int LEAF_THREADS = 128;
 // leaf r = sponge(row r of the concatenation of all committed matrices); `cols` holds one base pointer per column.
 // Overwrite-mode absorb, rate 8, no padding (PaddingFreeSponge<16,8,8>).  One thread per row; consecutive threads read
 // consecutive rows of a column-major matrix => every load is a fully coalesced 128 B warp transaction.
-#ifndef PB_V_LEAF_MINB
-#define PB_V_LEAF_MINB 1
-#endif
-__global__ void __launch_bounds__(256, PB_V_LEAF_MINB) leaf_hash_cols_kernel(const uint32_t* const* __restrict__ cols, uint32_t n_cols,
-                                                              size_t height, uint32_t* __restrict__ digests) {
+__global__ void __launch_bounds__(256, 1) leaf_hash_cols_kernel(const uint32_t* const* __restrict__ cols, uint32_t n_cols,
+                                                 size_t height, uint32_t* __restrict__ digests) {
     size_t r = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= height) return;
     uint32_t s[16];
 #pragma unroll
     for (int i = 0; i < 16; i++) s[i] = 0;
     uint32_t full = n_cols / 8;
-#ifdef PB_V_NOPREFETCH
-    for (uint32_t c = 0; c < full; c++) {
-#pragma unroll
-        for (int k = 0; k < 8; k++) s[k] = __ldg(cols[c * 8 + k] + r);
-        permute(s);
-    }
-#else
     uint32_t nxt[8];
     if (full) {
 #pragma unroll
@@ -184,7 +154,6 @@ __global__ void __launch_bounds__(256, PB_V_LEAF_MINB) leaf_hash_cols_kernel(con
         }
         permute(s);
     }
-#endif
     uint32_t rem = n_cols - full * 8;
     if (rem) {
 #pragma unroll
@@ -200,9 +169,9 @@ __global__ void __launch_bounds__(256, PB_V_LEAF_MINB) leaf_hash_cols_kernel(con
 // Streaming variant of the leaf sponge for the host-input pipeline: absorbs one CHUNK of columns (a multiple of 8 unless
 // it is the last chunk) into per-row sponge states kept in HBM as [16][height] (word-major => coalesced), so hashing of
 // chunk k overlaps the PCIe copy and the LDE of chunk k+1.  first: start from the zero state; last: emit the digest.
-__global__ void __launch_bounds__(256, PB_V_LEAF_MINB) leaf_absorb_cols_kernel(const uint32_t* const* __restrict__ cols, uint32_t n_cols, size_t height,
-                                                                uint32_t* __restrict__ state, uint32_t* __restrict__ digests,
-                                                                int first, int last) {
+__global__ void __launch_bounds__(256, 1) leaf_absorb_cols_kernel(const uint32_t* const* __restrict__ cols, uint32_t n_cols, size_t height,
+                                                   uint32_t* __restrict__ state, uint32_t* __restrict__ digests,
+                                                   int first, int last) {
     size_t r = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= height) return;
     uint32_t s[16];
@@ -446,10 +415,7 @@ __global__ void __launch_bounds__(32) fri_challenge_kernel(uint32_t* sponge16, c
 }
 
 // single permutation per thread on [n][16] states -- used by tests and the throughput micro-benchmark
-#ifndef PB_V_MINBLOCKS
-#define PB_V_MINBLOCKS 1
-#endif
-__global__ void __launch_bounds__(256, PB_V_MINBLOCKS) permute_states_kernel(uint32_t* states, size_t n, int reps) {
+__global__ void __launch_bounds__(256, 1) permute_states_kernel(uint32_t* states, size_t n, int reps) {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     uint32_t s[16];
