@@ -955,12 +955,18 @@ static int deep_quotient_groups_m(pb_ctx* ctx, const std::vector<const uint32_t*
     CK(cudaMemcpyAsync(ctx->ws_gp.p, gs.data(), gs.size() * sizeof(uint4), cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));           // gs is a host temporary
     struct Run { const uint32_t* base; size_t stride; uint32_t count, off, off2; };
+    // A group-0 run must start where a group-1 run starts: two matrices that happen to be adjacent in memory (the main LDE of one chip
+    // and the permutation LDE of the next) would otherwise merge into one run that no group-1 run mirrors.
+    std::vector<const uint32_t*> second_starts;
+    for (size_t j = 0; j < n_cols; j++)
+        if (grp[j] == 1 && (j == 0 || grp[j - 1] != 1)) second_starts.push_back(cols[j]);
+    auto starts_second = [&](const uint32_t* p) { return std::find(second_starts.begin(), second_starts.end(), p) != second_starts.end(); };
     std::vector<Run> runs;
     for (size_t j = 0; j < n_cols;) {
         if (grp[j] != 0) { j++; continue; }
         size_t k = j + 1;
         const ptrdiff_t st = (k < n_cols && grp[k] == 0) ? cols[k] - cols[j] : 0;
-        while (k < n_cols && grp[k] == 0 && st > 0 && cols[k] - cols[k - 1] == st) k++;
+        while (k < n_cols && grp[k] == 0 && st > 0 && cols[k] - cols[k - 1] == st && !starts_second(cols[k])) k++;
         if (st <= 0) k = j + 1;
         runs.push_back(Run{cols[j], st > 0 ? (size_t)st : 0, (uint32_t)(k - j), (uint32_t)j, deep::DQ_NO_SECOND});
         j = k;

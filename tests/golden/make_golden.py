@@ -18,6 +18,7 @@ reference-derived fixtures and the oracle for the generated vectors):  python te
                                    single_div_nondet, wasm_register_reuse and keccak_apc_pre_opt (677 instructions, 27 521 cells): the
                                    REAL stage-0 gather pattern (the machines of the big fixture are not committed: 28 627 constraints)
   chips_mixed.json                 three chips of different heights under one transcript (orc_prove_chips): proof, cumulative sums, digests
+  chips_tiny.json                  the same for 2-, 4- and 32-row chips with interactions: the bottom of the height range
   v1_metrics_reference.json        an OpenVM-1 metrics file written by powdr_b200.metrics and what the reference's own
                                    openvm-riscv/scripts/basic_metrics.py extracts from it (plots stubbed out: matplotlib is optional)
 """
@@ -123,11 +124,19 @@ def main():
     g.update(proof=proof, ys_sha256=sha(ys), queries_sha256=sha(q))
     dump("segment_logup_2p7.json", g)
 
-    g = {"spec": [[6, 12, 3, 7], [4, 9, 2, 0], [3, 10, 0, 3]], "seed": 5, "n_queries": 6, "pow_bits": 5}
+    chips_fixture("chips_mixed.json", [[6, 12, 3, 7], [4, 9, 2, 0], [3, 10, 0, 3]], seed=5, n_queries=6, pow_bits=5)
+    chips_fixture("chips_tiny.json", [[1, 6, 2, 3], [2, 7, 0, 4], [5, 9, 3, 2], [1, 5, 1, 0]], seed=7, n_queries=8, pow_bits=4)
+
+
+def chips_fixture(name, spec, seed, n_queries, pow_bits):
+    """a multi-chip proof by the oracle: proof fields, cumulative sums, digests of the opened values and query words"""
+    import hashlib
+    sha = lambda a: hashlib.sha256(np.ascontiguousarray(a, dtype=np.uint32).tobytes()).hexdigest()
+    g = {"spec": spec, "seed": seed, "n_queries": n_queries, "pow_bits": pow_bits}
     chips = chips_for(g["spec"], g["seed"])
     proof, cs, ys, q = orc.prove_chips(chips, n_queries=g["n_queries"], pow_bits=g["pow_bits"])
     g.update(proof=proof, cumsums=cs.tolist(), ys_sha256=sha(ys), queries_sha256=sha(q))
-    dump("chips_mixed.json", g)
+    dump(name, g)
 
 
 METRICS_STAGES_MS = {"h2d": 0.1, "lde": 34.0, "merkle": 130.0, "logup_gen": 46.0, "logup_commit": 270.0, "quotient": 60.0, "qlde": 0.3,

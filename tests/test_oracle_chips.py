@@ -108,7 +108,7 @@ def test_random_chip_mixes_verify_and_bind_every_opened_value(orc):
 
 
 def test_committed_fixtures_are_reproduced(orc):
-    """tests/golden/segment_logup_2p7.json and chips_mixed.json (written by tests/golden/make_golden.py): regression pins of transcript
+    """tests/golden/segment_logup_2p7.json, chips_mixed.json and chips_tiny.json (written by tests/golden/make_golden.py): regression pins of transcript
     v2 with the LogUp phase and of the multi-chip transcript -- proof fields exactly, opened values / query openings by digest"""
     import hashlib
     import json
@@ -127,9 +127,10 @@ def test_committed_fixtures_are_reproduced(orc):
     for fast in ([False, True] if orc.fast_available() else [False]):
         proof, ys, q, _ = orc.prove(trace, bc, spans, M.compile_bus(mach, 1), n_queries=g["n_queries"], pow_bits=g["pow_bits"], fast=fast)
         assert proof == g["proof"] and sha(ys) == g["ys_sha256"] and sha(q) == g["queries_sha256"]
-    g = json.load(open(os.path.join(golden, "chips_mixed.json")))
-    chips = chips_for([tuple(x) for x in g["spec"]], g["seed"])
-    for fast in ([False, True] if orc.fast_available() else [False]):
-        proof, cs, ys, q = orc.prove_chips(chips, n_queries=g["n_queries"], pow_bits=g["pow_bits"], fast=fast)
-        assert proof == g["proof"] and cs.tolist() == g["cumsums"] and sha(ys) == g["ys_sha256"] and sha(q) == g["queries_sha256"]
-    assert orc.verify_chips(chips, proof, cs, ys, q, check_constraints=False) == 0
+    for name in ("chips_mixed.json", "chips_tiny.json"):          # chips_tiny: 2-, 4- and 32-row chips, the bottom of the height range
+        g = json.load(open(os.path.join(golden, name)))
+        chips = chips_for([tuple(x) for x in g["spec"]], g["seed"])
+        for fast in ([False, True] if orc.fast_available() else [False]):
+            proof, cs, ys, q = orc.prove_chips(chips, n_queries=g["n_queries"], pow_bits=g["pow_bits"], fast=fast)
+            assert proof == g["proof"] and cs.tolist() == g["cumsums"] and sha(ys) == g["ys_sha256"] and sha(q) == g["queries_sha256"], name
+        assert orc.verify_chips(chips, proof, cs, ys, q, check_constraints=False) == 0
