@@ -537,23 +537,21 @@ void orcf_eval_at_point(const uint32_t* mat, unsigned log_n, size_t width, uint3
     free(ws);
 }
 
-/* reduced opening, general form used by the segment prover:
- *   ro[r] = sum_g ( sum_{j in group g} gamma^(e0_g + j) * (f_j[r] - y_{g,j}) ) / (x_r - z_g),  x_r = shift * w_m^{bitrev(r)}.
- * A group = a run of columns opened at one point.  ys: per group [n_cols][4].  out [m][4]. */
+/* reduced opening, general form used by the prover:
+ *   ro[r] = sum_g ( sum_{j in group g} gamma_j * (f_j[r] - y_j) ) / (x_r - z_g),  x_r = shift * w_m^{bitrev(r)}.
+ * A group = the columns opened at one point; gamma_j = the column's power of the batching challenge.  out [m][4]. */
 void orcf_deep_quotient_groups(const uint32_t* const* cols, const uint32_t* group_of_col, size_t n_cols, const uint32_t* zs /*[G][4]*/,
-                               size_t n_groups, unsigned log_m, uint32_t shift, const uint32_t gamma[4], const uint32_t* ys /*[n_cols][4]*/,
-                               uint32_t* out) {
+                               size_t n_groups, unsigned log_m, uint32_t shift, const uint32_t* gamma_pows /*[n_cols][4]*/,
+                               const uint32_t* ys /*[n_cols][4]*/, uint32_t* out) {
     const size_t m = (size_t)1 << log_m;
-    bb4_t g = {{gamma[0], gamma[1], gamma[2], gamma[3]}};
-    uint32_t* gp = (uint32_t*)malloc((n_cols ? n_cols : 1) * 16);           /* Montgomery limbs of gamma^j */
+    uint32_t* gp = (uint32_t*)malloc((n_cols ? n_cols : 1) * 16);           /* Montgomery limbs of gamma_j */
     bb4_t* ysum = (bb4_t*)calloc(n_groups, sizeof(bb4_t));
-    bb4_t cur = bb4_from_base(1);
     for (size_t j = 0; j < n_cols; j++) {
-        for (int l = 0; l < 4; l++) gp[4 * j + l] = to_m(cur.c[l]);
-        bb4_t y;
+        for (int l = 0; l < 4; l++) gp[4 * j + l] = to_m(gamma_pows[4 * j + l]);
+        bb4_t gj, y;
+        memcpy(gj.c, gamma_pows + 4 * j, 16);
         memcpy(y.c, ys + 4 * j, 16);
-        ysum[group_of_col[j]] = bb4_add(ysum[group_of_col[j]], bb4_mul(cur, y));
-        cur = bb4_mul(cur, g);
+        ysum[group_of_col[j]] = bb4_add(ysum[group_of_col[j]], bb4_mul(gj, y));
     }
     const uint32_t w = bb_root_of_unity(log_m);
     bb4_t* acc_all = (bb4_t*)malloc(n_groups * m * sizeof(bb4_t));         /* numerators per group, canonical */
@@ -579,11 +577,13 @@ void orcf_deep_quotient_groups(const uint32_t* const* cols, const uint32_t* grou
     } else {
         for (size_t r = 0; r < m; r++)
             for (size_t q = 0; q < n_groups; q++) {
-                bb4_t a = bb4_from_base(0), c = bb4_from_base(1);
-                for (size_t j = 0; j < n_cols; j++) {
-                    if (group_of_col[j] == q) a = bb4_add(a, bb4_scale(c, cols[j][r]));
-                    c = bb4_mul(c, g);
-                }
+                bb4_t a = bb4_from_base(0);
+                for (size_t j = 0; j < n_cols; j++)
+                    if (group_of_col[j] == q) {
+                        bb4_t gj;
+                        memcpy(gj.c, gamma_pows + 4 * j, 16);
+                        a = bb4_add(a, bb4_scale(gj, cols[j][r]));
+                    }
                 acc_all[q * m + r] = bb4_sub(a, ysum[q]);
             }
     }
@@ -621,10 +621,14 @@ void orcf_deep_quotient(const uint32_t* const* mats, const size_t* widths, size_
     for (size_t i = 0; i < n_mats; i++) total += widths[i];
     const uint32_t** cols = (const uint32_t**)malloc((total ? total : 1) * sizeof(*cols));
     uint32_t* grp = (uint32_t*)calloc(total ? total : 1, sizeof(uint32_t));
+    uint32_t* gp = (uint32_t*)malloc((total ? total : 1) * 16);               /* consecutive powers gamma^0, gamma^1, ... */
     size_t k = 0;
     for (size_t i = 0; i < n_mats; i++) for (size_t c = 0; c < widths[i]; c++) cols[k++] = mats[i] + c * m;
-    orcf_deep_quotient_groups(cols, grp, total, zeta, 1, log_m, shift, gamma, ys, out);
-    free(cols); free(grp);
+    bb4_t cur = bb4_from_base(1);
+    const bb4_t g = {{gamma[0], gamma[1], gamma[2], gamma[3]}};
+    for (size_t j = 0; j < total; j++) { memcpy(gp + 4 * j, cur.c, 16); cur = bb4_mul(cur, g); }
+    orcf_deep_quotient_groups(cols, grp, total, zeta, 1, log_m, shift, gp, ys, out);
+    free(cols); free(grp); free(gp);
 }
 
 /* =====================================================================================================================

@@ -164,21 +164,18 @@ void orc_deep_quotient(const uint32_t* const* mats, const size_t* widths, size_t
 }
 
 /* reduced opening over several (column group, point) pairs:
-   ro[r] = sum_g ( sum_{j in g} gamma^j * (f_j[r] - y_j) ) / (x_r - z_g),  j = the column's global index in `cols` (= its exponent).
-   cols[j]: one column of height 2^log_m (bit-reversed rows over shift*H'); ys: [n_cols][4]; zs: [n_groups][4]; out [m][4]. */
+   ro[r] = sum_g ( sum_{j in g} gamma_j * (f_j[r] - y_j) ) / (x_r - z_g),  gamma_j = the column's power of the batching challenge.
+   cols[j]: one column of height 2^log_m (bit-reversed rows over shift*H'); gamma_pows, ys: [n_cols][4]; zs: [n_groups][4]; out [m][4]. */
 void orc_deep_quotient_groups(const uint32_t* const* cols, const uint32_t* group_of_col, size_t n_cols, const uint32_t* zs, size_t n_groups,
-                              unsigned log_m, uint32_t shift, const uint32_t gamma[4], const uint32_t* ys, uint32_t* out) {
+                              unsigned log_m, uint32_t shift, const uint32_t* gamma_pows, const uint32_t* ys, uint32_t* out) {
     const size_t m = (size_t)1 << log_m;
-    bb4_t g = {{gamma[0], gamma[1], gamma[2], gamma[3]}};
     bb4_t* gp = (bb4_t*)malloc((n_cols ? n_cols : 1) * sizeof(bb4_t));
     bb4_t* ysum = (bb4_t*)calloc(n_groups, sizeof(bb4_t));
-    bb4_t cur = bb4_from_base(1);
     for (size_t j = 0; j < n_cols; j++) {
-        gp[j] = cur;
         bb4_t y;
+        memcpy(gp[j].c, gamma_pows + 4 * j, 16);
         memcpy(y.c, ys + 4 * j, 16);
-        ysum[group_of_col[j]] = bb4_add(ysum[group_of_col[j]], bb4_mul(cur, y));
-        cur = bb4_mul(cur, g);
+        ysum[group_of_col[j]] = bb4_add(ysum[group_of_col[j]], bb4_mul(gp[j], y));
     }
     const uint32_t w = bb_root_of_unity(log_m);
 #pragma omp parallel for schedule(static)

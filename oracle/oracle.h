@@ -91,13 +91,14 @@ void orc_logup_perm_trace(const uint32_t* trace, unsigned log_n, const uint32_t*
 void orc_logup_fold(const uint32_t* lde, const uint32_t* perm_lde, unsigned log_n, uint32_t shift, const uint32_t* ibc, const orc_span_t* isp,
                     const orc_interaction_t* ints, size_t n_ints, const uint32_t* chunk_start, size_t n_chunks, const uint32_t alpha_lu[4],
                     const uint32_t beta_lu[4], const uint32_t cumsum[4], const uint32_t alpha[4], uint32_t* acc4 /* [4][2N] in/out */);
-/* reduced opening over several (column group, point) pairs -- see ntt.c */
+/* reduced opening over several (column group, point) pairs, column j weighted by gamma_pows[j] -- see ntt.c */
 void orc_deep_quotient_groups(const uint32_t* const* cols, const uint32_t* group_of_col, size_t n_cols, const uint32_t* zs, size_t n_groups,
-                              unsigned log_m, uint32_t shift, const uint32_t gamma[4], const uint32_t* ys, uint32_t* out);
+                              unsigned log_m, uint32_t shift, const uint32_t* gamma_pows, const uint32_t* ys, uint32_t* out);
 
-/* ---- whole segment (the metric's unit of work), transcript v2 (DESIGN.md §3) ----
-   main commit -> [LogUp challenges, permutation trace commit, cumulative sum] -> alpha -> quotient commit -> zeta ->
-   openings (every opened value observed) -> gamma -> FRI commit phase -> final polynomial observed -> proof-of-work -> queries */
+/* ---- all chips of a segment (the metric's unit of work) under ONE transcript, v2 (DESIGN.md §3, §3b; prove.c, verify.c) ----
+   main commit -> [LogUp challenges, permutation trace commit, cumulative sums] -> alpha -> quotient commit -> zeta ->
+   openings (every opened value observed) -> gamma -> FRI commit phase -> final polynomial observed -> proof-of-work -> queries.
+   Mixed-height MMCS commitments, shared challenges, one FRI instance.  A single segment is a one-chip proof. */
 typedef struct {
     const uint32_t* bc; const orc_span_t* spans; size_t n_constraints;                              /* polynomial identities */
     const uint32_t* ibc; const orc_span_t* ispans; const orc_interaction_t* ints; size_t n_ints;   /* bus interactions (may be 0) */
@@ -107,62 +108,35 @@ typedef struct {
     int fast;             /* 1: AVX-512 primitives of fast.c where available */
     int cheat_opening;    /* test hook: a dishonest prover that claims main_col0(zeta) + 1 -- its reduced opening is not a polynomial */
 } orc_params_t;
+size_t orc_perm_width(const orc_air_t* air);
+/* proof-of-work grinding on a challenger state: smallest witness w with (observe(w); sample() & (2^bits - 1)) == 0 */
+uint32_t orc_grind(const orc_challenger_t* c, unsigned bits);
+typedef struct { const orc_air_t* air; const uint32_t* trace; unsigned log_n; size_t width; } orc_chip_t;
 typedef struct {
-    uint32_t trace_root[8];
-    uint32_t logup_alpha[4], logup_beta[4];   /* zero when the AIR has no interactions */
-    uint32_t perm_root[8];
-    uint32_t cumulative_sum[4];
-    uint32_t alpha[4];
-    uint32_t quotient_root[8];
-    uint32_t zeta[4];              /* out-of-domain opening point */
-    uint32_t gamma[4];             /* batching challenge of the reduced opening */
+    uint32_t main_root[8], perm_root[8], quotient_root[8];
+    uint32_t logup_alpha[4], logup_beta[4];        /* zero when no chip has interactions */
+    uint32_t alpha[4], zeta[4] /* out-of-domain opening point */, gamma[4] /* batching challenge of the reduced opening */;
     uint32_t n_fri_layers;
     uint32_t fri_roots[32][8];
     uint32_t fri_betas[32][4];
     uint32_t final_poly[8][4];     /* last layer (length 2^log_blowup): evaluations of the constant final polynomial */
     uint32_t final_len;
     uint32_t pow_witness;
-    uint32_t pow_bits, n_queries, perm_width;
-} orc_segment_proof_t;
-/* opened values ys: [(width + 2*perm_width + 8)][4] = main at zeta | perm at zeta | perm at zeta*w | quotient chunks at zeta.
-   query layout (words): [ r | main row | main path | perm row | perm path (both absent when perm_width = 0) | quotient row (8) |
-   quotient path | per FRI layer: pair (8), path ] */
-size_t orc_num_opened(size_t width, size_t perm_width);
-size_t orc_query_words(unsigned log_n, size_t width, size_t perm_width);
-size_t orc_perm_width(const orc_air_t* air);
-/* stage_seconds[10]: lde, merkle, logup_gen, logup_commit, quotient, quotient_commit, openings, fri_commit, pow, query */
-void orc_prove_segment(const uint32_t* trace, unsigned log_n, size_t width, const orc_air_t* air, const orc_params_t* prm,
-                       orc_segment_proof_t* proof, double stage_seconds[10], uint32_t* ys_out, uint32_t* queries_out);
-/* independent verifier; 0 = accept, else the failed check:
-   1 logup challenges 2 alpha 3 zeta 4 gamma 5 beta 6 proof of work 7 query index 8 main path 9 perm path 10 quotient path
-   11 reduced opening != FRI layer 0 12 FRI path 13 fold consistency 14 final polynomial value 15 final polynomial not constant
-   16 constraint identity at zeta 20 malformed */
-int orc_verify_segment(const orc_air_t* air, unsigned log_n, size_t width, const orc_segment_proof_t* proof, const uint32_t* ys,
-                       const uint32_t* queries, int check_constraints);
-/* proof-of-work grinding on a challenger state: smallest witness w with (observe(w); sample() & (2^bits - 1)) == 0 */
-uint32_t orc_grind(const orc_challenger_t* c, unsigned bits);
-
-/* ---- multi-chip segment under ONE transcript (prove.c, verify.c): mixed-height MMCS commitments, shared challenges, one FRI ---- */
-typedef struct { const orc_air_t* air; const uint32_t* trace; unsigned log_n; size_t width; } orc_chip_t;
-typedef struct {
-    uint32_t main_root[8], perm_root[8], quotient_root[8];
-    uint32_t logup_alpha[4], logup_beta[4], alpha[4], zeta[4], gamma[4];
-    uint32_t n_fri_layers;
-    uint32_t fri_roots[32][8];
-    uint32_t fri_betas[32][4];
-    uint32_t final_poly[8][4];
-    uint32_t final_len;
-    uint32_t pow_witness;
     uint32_t pow_bits, n_queries, n_chips, log_max;       /* log_max: log2 of the tallest LDE */
 } orc_chips_proof_t;
 size_t orc_chips_num_opened(const orc_chip_t* chips, size_t n_chips);
 size_t orc_chips_query_words(const orc_chip_t* chips, size_t n_chips);
-/* cumsums: [n_chips][4] (zero for chips without interactions); ys_out: [orc_chips_num_opened][4]; queries_out: [n_queries][orc_chips_query_words].
+/* cumsums: [n_chips][4] (zero for chips without interactions); ys_out: [orc_chips_num_opened][4] = main at zeta (chip order) | per chip with
+   interactions perm at zeta, perm at zeta*w_chip | quotient chunks at zeta (chip order); queries_out: [n_queries][orc_chips_query_words].
    query layout: [ r | main rows of all chips (row r >> (log_max - log_m_chip)) | main path (log_max x 8) | perm rows of the chips with
-   interactions | perm path | quotient rows (8 per chip) | quotient path | per FRI layer: pair (8), path ] */
+   interactions | perm path (both absent when no chip has interactions) | quotient rows (8 per chip) | quotient path | per FRI layer: pair (8), path ]
+   stage_seconds[10] (NULL: not clocked): lde, merkle, logup_gen, logup_commit, quotient, quotient_commit, openings, fri_commit, pow, query */
 void orc_prove_chips(const orc_chip_t* chips, size_t n_chips, const orc_params_t* prm, orc_chips_proof_t* proof, uint32_t* cumsums, uint32_t* ys_out,
-                     uint32_t* queries_out);
-/* 0 = accept; codes as orc_verify_segment (8/9/10 = main/perm/quotient MMCS opening) */
+                     uint32_t* queries_out, double stage_seconds[10]);
+/* independent verifier (only the shapes of the chips are read, not their traces); 0 = accept, else the failed check:
+   1 logup challenges 2 alpha 3 zeta 4 gamma 5 beta 6 proof of work 7 query index 8 main path 9 perm path 10 quotient path
+   (8/9/10: MMCS openings) 11 reduced opening != FRI layer 0 12 FRI path 13 fold consistency 14 final polynomial value
+   15 final polynomial not constant 16 constraint identity at zeta 20 malformed */
 int orc_verify_chips(const orc_chip_t* chips_without_traces, size_t n_chips, const orc_chips_proof_t* proof, const uint32_t* cumsums, const uint32_t* ys,
                      const uint32_t* queries, int check_constraints);
 
@@ -184,7 +158,7 @@ void orcf_logup_fold(const uint32_t* lde, const uint32_t* perm_lde, unsigned log
                      const orc_interaction_t* ints, size_t n_ints, const uint32_t* chunk_start, size_t n_chunks, const uint32_t alpha_lu[4],
                      const uint32_t beta_lu[4], const uint32_t cumsum[4], const uint32_t alpha[4], uint32_t* acc4);
 void orcf_deep_quotient_groups(const uint32_t* const* cols, const uint32_t* group_of_col, size_t n_cols, const uint32_t* zs, size_t n_groups,
-                               unsigned log_m, uint32_t shift, const uint32_t gamma[4], const uint32_t* ys, uint32_t* out);
+                               unsigned log_m, uint32_t shift, const uint32_t* gamma_pows, const uint32_t* ys, uint32_t* out);
 int orc_num_threads(void);
 void* orc_big_alloc(size_t bytes);   /* 2 MB aligned, MADV_HUGEPAGE */
 void orc_big_free(void* p);

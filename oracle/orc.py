@@ -42,44 +42,6 @@ class Interaction(C.Structure):
     _fields_ = [("bus_id", C.c_uint32), ("num_args", C.c_uint32), ("args_index_off", C.c_uint32)]
 
 
-class SegmentProof(C.Structure):
-    _fields_ = [("trace_root", C.c_uint32 * 8), ("logup_alpha", C.c_uint32 * 4), ("logup_beta", C.c_uint32 * 4),
-                ("perm_root", C.c_uint32 * 8), ("cumulative_sum", C.c_uint32 * 4), ("alpha", C.c_uint32 * 4),
-                ("quotient_root", C.c_uint32 * 8), ("zeta", C.c_uint32 * 4), ("gamma", C.c_uint32 * 4),
-                ("n_fri_layers", C.c_uint32), ("fri_roots", (C.c_uint32 * 8) * 32), ("fri_betas", (C.c_uint32 * 4) * 32),
-                ("final_poly", (C.c_uint32 * 4) * 8), ("final_len", C.c_uint32), ("pow_witness", C.c_uint32),
-                ("pow_bits", C.c_uint32), ("n_queries", C.c_uint32), ("perm_width", C.c_uint32)]
-    VEC = ("trace_root", "logup_alpha", "logup_beta", "perm_root", "cumulative_sum", "alpha", "quotient_root", "zeta", "gamma")
-    SCALAR = ("n_fri_layers", "final_len", "pow_witness", "pow_bits", "n_queries", "perm_width")
-
-    def as_dict(self):
-        n = self.n_fri_layers
-        d = {k: list(getattr(self, k)) for k in self.VEC}
-        d.update({k: int(getattr(self, k)) for k in self.SCALAR})
-        d["fri_roots"] = [list(self.fri_roots[i]) for i in range(n)]
-        d["fri_betas"] = [list(self.fri_betas[i]) for i in range(n)]
-        d["final_poly"] = [list(self.final_poly[i]) for i in range(self.final_len)]
-        return d
-
-    @classmethod
-    def from_dict(cls, d):
-        p = cls()
-        for k in cls.VEC:
-            for i, v in enumerate(d[k]):
-                getattr(p, k)[i] = v
-        for k in cls.SCALAR:
-            setattr(p, k, d[k])
-        for i in range(d["n_fri_layers"]):
-            for j in range(8):
-                p.fri_roots[i][j] = d["fri_roots"][i][j]
-            for j in range(4):
-                p.fri_betas[i][j] = d["fri_betas"][i][j]
-        for i in range(d["final_len"]):
-            for j in range(4):
-                p.final_poly[i][j] = d["final_poly"][i][j]
-        return p
-
-
 class AirC(C.Structure):
     _fields_ = [("bc", C.c_void_p), ("spans", C.c_void_p), ("n_constraints", C.c_size_t),
                 ("ibc", C.c_void_p), ("ispans", C.c_void_p), ("ints", C.c_void_p), ("n_ints", C.c_size_t)]
@@ -331,50 +293,6 @@ def apc_apply_bus(out, num_calls, bc, interactions, arg_spans, var=(3, 1 << 18),
     return var_hist, t_hist, b_hist
 
 
-STAGES = ("lde", "merkle", "logup_gen", "logup_commit", "quotient", "quotient_commit", "openings", "fri_commit", "pow", "query")
-
-
-def query_words(log_n, width, perm_width=0):
-    lib().orc_query_words.restype = C.c_size_t
-    return int(lib().orc_query_words(C.c_uint(log_n), C.c_size_t(width), C.c_size_t(perm_width)))
-
-
-def prove(trace, bc, spans, bus=None, n_queries=8, pow_bits=4, fast=False, cheat_opening=False):
-    """-> (proof dict, opened values (n_open, 4), query openings (n_queries, words), {stage: seconds})"""
-    t = _u32(trace)
-    w, n = t.shape
-    log_n = n.bit_length() - 1
-    air = bus if isinstance(bus, Air) else Air(bc, spans, bus)
-    wp = air.perm_width
-    proof = SegmentProof()
-    st = (C.c_double * 10)()
-    ys = np.empty((w + 2 * wp + 8, 4), dtype=np.uint32)
-    q = np.empty((n_queries, query_words(log_n, w, wp)), dtype=np.uint32)
-    prm = ParamsC(n_queries, pow_bits, 1 if fast else 0, 1 if cheat_opening else 0)
-    lib().orc_prove_segment(_p(t), C.c_uint(log_n), C.c_size_t(w), C.byref(air.c), C.byref(prm), C.byref(proof), st, _p(ys), _p(q))
-    return proof.as_dict(), ys, q, dict(zip(STAGES, list(st)))
-
-
-def prove_segment(trace, bc, spans, bus=None, n_queries=8, pow_bits=4, fast=False):
-    d, _, _, st = prove(trace, bc, spans, bus, n_queries, pow_bits, fast)
-    return d, st
-
-
-def prove_segment_q(trace, bc, spans, n_queries, bus=None, pow_bits=4, fast=False):
-    d, ys, q, _ = prove(trace, bc, spans, bus, n_queries, pow_bits, fast)
-    return d, ys, q
-
-
-def verify_segment(bc, spans, log_n, width, proof, ys, queries, check_constraints=False, bus=None):
-    """0 = accept; see oracle.h for the failure codes"""
-    air = bus if isinstance(bus, Air) else Air(bc, spans, bus)
-    ys, q = _u32(ys), _u32(queries)
-    p = SegmentProof.from_dict(proof)
-    lib().orc_verify_segment.restype = C.c_int
-    return lib().orc_verify_segment(C.byref(air.c), C.c_uint(log_n), C.c_size_t(width), C.byref(p), _p(ys), _p(q),
-                                    C.c_int(1 if check_constraints else 0))
-
-
 def grind(challenger, bits):
     lib().orc_grind.restype = C.c_uint32
     return int(lib().orc_grind(C.byref(challenger.s), C.c_uint(bits)))
@@ -514,23 +432,27 @@ class ChipsProof(C.Structure):
 
 
 def _chips_array(chips):
-    """chips: list of (trace (W, N) or None, bc, spans, bus) -> (ctypes array, keep-alive list)"""
+    """chips: list of (trace (W, N), bc, spans, bus) -> (ctypes array, keep-alive list).  bus may already be an Air; for the verifier,
+    which reads only the shape, the trace may be given as its shape (W, N)."""
     arr = (ChipC * len(chips))()
     keep = []
     for i, (trace, bc, spans, bus) in enumerate(chips):
-        air = Air(bc, spans, bus)
-        t = _u32(trace) if trace is not None else None
+        air = bus if isinstance(bus, Air) else Air(bc, spans, bus)
+        t = None if isinstance(trace, tuple) else _u32(trace)
         keep.append((air, t))
+        w, n = trace if t is None else t.shape
         arr[i].air = C.addressof(air.c)
-        arr[i].trace = t.ctypes.data if t is not None else None
-        w, n = (t.shape if t is not None else (0, 0))
-        arr[i].log_n = (n.bit_length() - 1) if t is not None else 0
+        arr[i].trace = None if t is None else t.ctypes.data
+        arr[i].log_n = n.bit_length() - 1
         arr[i].width = w
     return arr, keep
 
 
-def prove_chips(chips, n_queries=8, pow_bits=4, fast=False):
-    """chips: list of (trace, bc, spans, bus) -> (proof dict, cumulative sums (K, 4), opened values (n_open, 4), queries (n_queries, words))"""
+STAGES = ("lde", "merkle", "logup_gen", "logup_commit", "quotient", "quotient_commit", "openings", "fri_commit", "pow", "query")
+
+
+def _prove(chips, n_queries, pow_bits, fast, cheat_opening=False):
+    """-> (ChipsProof, cumulative sums (K, 4), opened values (n_open, 4), queries (n_queries, words), {stage: seconds})"""
     arr, keep = _chips_array(chips)
     K = len(chips)
     L = lib()
@@ -542,15 +464,61 @@ def prove_chips(chips, n_queries=8, pow_bits=4, fast=False):
     cs = np.zeros((K, 4), dtype=np.uint32)
     ys = np.empty((n_open, 4), dtype=np.uint32)
     q = np.empty((n_queries, wpq), dtype=np.uint32)
-    prm = ParamsC(n_queries, pow_bits, 1 if fast else 0, 0)
-    L.orc_prove_chips(arr, C.c_size_t(K), C.byref(prm), C.byref(proof), _p(cs), _p(ys), _p(q))
+    st = (C.c_double * 10)()
+    prm = ParamsC(n_queries, pow_bits, 1 if fast else 0, 1 if cheat_opening else 0)
+    L.orc_prove_chips(arr, C.c_size_t(K), C.byref(prm), C.byref(proof), _p(cs), _p(ys), _p(q), st)
+    return proof, cs, ys, q, dict(zip(STAGES, list(st)))
+
+
+def prove_chips(chips, n_queries=8, pow_bits=4, fast=False):
+    """chips: list of (trace, bc, spans, bus) -> (proof dict, cumulative sums (K, 4), opened values (n_open, 4), queries (n_queries, words))"""
+    proof, cs, ys, q, _ = _prove(chips, n_queries, pow_bits, fast)
     return proof.as_dict(), cs, ys, q
 
 
 def verify_chips(chips, proof, cumsums, ys, queries, check_constraints=False):
-    """chips: list of (trace-or-shape, bc, spans, bus); only the shape of the trace is used"""
+    """chips: list of (trace-or-shape, bc, spans, bus); only the shape of the trace is used.  0 = accept; see oracle.h for the failure codes"""
     arr, keep = _chips_array(chips)
     p = ChipsProof.from_dict(proof)
     cs, ys, q = _u32(cumsums), _u32(ys), _u32(queries)
     lib().orc_verify_chips.restype = C.c_int
     return lib().orc_verify_chips(arr, C.c_size_t(len(chips)), C.byref(p), _p(cs), _p(ys), _p(q), C.c_int(1 if check_constraints else 0))
+
+
+# ---- a single segment: the one-chip proof, as the dict the GPU prover returns and the fixtures pin ----
+SEGMENT_KEYS = ("trace_root", "logup_alpha", "logup_beta", "perm_root", "cumulative_sum", "alpha", "quotient_root", "zeta", "gamma",
+                "n_fri_layers", "final_len", "pow_witness", "pow_bits", "n_queries", "perm_width", "fri_roots", "fri_betas", "final_poly")
+
+
+def query_words(log_n, width, perm_width=0):
+    """words per query of a single segment: r | main row, path | perm row, path (when perm_width) | quotient row, path | FRI layers"""
+    log_m = log_n + 1
+    return (1 + width + 8 * log_m + (perm_width + 8 * log_m if perm_width else 0) + 8 + 8 * log_m +
+            sum(8 + 8 * (log_m - 1 - i) for i in range(log_n)))
+
+
+def prove(trace, bc, spans, bus=None, n_queries=8, pow_bits=4, fast=False, cheat_opening=False):
+    """-> (proof dict, opened values (n_open, 4), query openings (n_queries, words), {stage: seconds})"""
+    air = bus if isinstance(bus, Air) else Air(bc, spans, bus)
+    proof, cs, ys, q, st = _prove([(trace, bc, spans, air)], n_queries, pow_bits, fast, cheat_opening)
+    d = dict(proof.as_dict(), trace_root=list(proof.main_root), cumulative_sum=cs[0].tolist(), perm_width=air.perm_width)
+    return {k: d[k] for k in SEGMENT_KEYS}, ys, q, st
+
+
+def prove_segment(trace, bc, spans, bus=None, n_queries=8, pow_bits=4, fast=False):
+    d, _, _, st = prove(trace, bc, spans, bus, n_queries, pow_bits, fast)
+    return d, st
+
+
+def prove_segment_q(trace, bc, spans, n_queries, bus=None, pow_bits=4, fast=False):
+    d, ys, q, _ = prove(trace, bc, spans, bus, n_queries, pow_bits, fast)
+    return d, ys, q
+
+
+def verify_segment(bc, spans, log_n, width, proof, ys, queries, check_constraints=False, bus=None):
+    """0 = accept; see oracle.h for the failure codes"""
+    air = bus if isinstance(bus, Air) else Air(bc, spans, bus)
+    if proof["perm_width"] != air.perm_width:
+        return 20
+    chips_proof = dict(proof, main_root=proof["trace_root"], n_chips=1, log_max=log_n + 1)
+    return verify_chips([((width, 1 << log_n), bc, spans, air)], chips_proof, [proof["cumulative_sum"]], ys, queries, check_constraints)

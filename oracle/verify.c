@@ -1,12 +1,15 @@
 /*
- * ORACLE (test infrastructure, not product code): an independent VERIFIER for the segment proof object.
+ * ORACLE (test infrastructure, not product code): an independent VERIFIER for the segment proof object of orc_prove_chips
+ * (all chips of a segment under one transcript; a single segment is one chip).
  * The reference's own tests pin the prover only by validity -- a proof produced by engine E must verify under the CPU
  * engine (verify_app_proof::<BabyBearPoseidon2CpuEngine>, /root/reference/openvm-riscv/src/lib.rs:337-341; SURVEY.md §4).
- * This file plays that role for the transcript v2 of DESIGN.md §3: it re-derives every challenge (LogUp, alpha, zeta, gamma,
- * betas), checks the proof of work, recomputes the reduced opening (two opening points) from the opened rows, checks every
- * Merkle path, every FRI fold, that the final polynomial is CONSTANT and matches, and (optionally, for satisfying traces) the
- * constraint identity  Horner_alpha(c_k(T(zeta)), LogUp constraints at zeta) = Z_H(zeta) * Q(zeta).
- * It shares no state with the prover: inputs are the proof struct, the opened values and the query openings.
+ * This file plays that role for the transcript v2 of DESIGN.md §3, §3b: it re-derives every challenge (LogUp, alpha, zeta, gamma,
+ * betas), checks the proof of work, checks every mixed-height MMCS opening, recomputes the reduced opening of each LDE height (two
+ * opening points) from the opened rows, checks every FRI path and fold with the per-height injection of the reduced openings, that
+ * the final polynomial is CONSTANT and matches, and (optionally, for satisfying traces) per chip the constraint identity
+ * Horner_alpha(c_k(T(zeta)), LogUp constraints at zeta) = Z_H(zeta) * Q(zeta).
+ * It shares no code or state with the prover: inputs are the chip shapes, the proof struct, the cumulative sums, the opened values
+ * and the query openings.
  */
 #include "oracle.h"
 #include "bb31.h"
@@ -50,179 +53,7 @@ bb4_t orc_logup_fold_at_point(bb4_t acc, bb4_t alpha, const uint32_t* main_ys, c
                               unsigned log_n, bb4_t zeta, const uint32_t* ibc, const orc_span_t* isp, const orc_interaction_t* ints, size_t n_ints,
                               const uint32_t* chunk_start, size_t n_chunks, bb4_t al, const uint32_t beta_lu[4], bb4_t cumsum);
 
-int orc_verify_segment(const orc_air_t* air, unsigned log_n, size_t width, const orc_segment_proof_t* proof, const uint32_t* ys,
-                       const uint32_t* queries, int check_constraints) {
-    const unsigned log_m = log_n + 1;
-    const size_t n = (size_t)1 << log_n;
-    if (proof->n_fri_layers != log_n || proof->final_len != 2) return 20;
-    size_t n_chunks = 0, wp = 0;
-    uint32_t* chunk_start = NULL;
-    if (air->n_ints) {
-        chunk_start = (uint32_t*)malloc((air->n_ints + 1) * sizeof(uint32_t));
-        int nc = orc_logup_chunks(air->ibc, air->ispans, air->ints, air->n_ints, 3, chunk_start);
-        if (nc < 0) { free(chunk_start); return 20; }
-        n_chunks = (size_t)nc;
-        wp = 4 * (n_chunks + 1);
-    }
-    if (proof->perm_width != wp) { free(chunk_start); return 20; }
-    const size_t n_open = orc_num_opened(width, wp);
-    const size_t n_queries = proof->n_queries;
-    int rc = 0;
-#define FAIL(code) do { rc = (code); goto done; } while (0)
-    bb4_t* gp = NULL;
-
-    /* 1. transcript */
-    orc_challenger_t ch;
-    orc_challenger_init(&ch);
-    uint32_t t4[4];
-    orc_challenger_observe(&ch, proof->trace_root, 8);
-    if (air->n_ints) {
-        orc_challenger_sample_ext(&ch, t4);
-        if (memcmp(t4, proof->logup_alpha, 16)) FAIL(1);
-        orc_challenger_sample_ext(&ch, t4);
-        if (memcmp(t4, proof->logup_beta, 16)) FAIL(1);
-        orc_challenger_observe(&ch, proof->perm_root, 8);
-        orc_challenger_observe(&ch, proof->cumulative_sum, 4);
-    }
-    orc_challenger_sample_ext(&ch, t4);
-    if (memcmp(t4, proof->alpha, 16)) FAIL(2);
-    orc_challenger_observe(&ch, proof->quotient_root, 8);
-    orc_challenger_sample_ext(&ch, t4);
-    if (memcmp(t4, proof->zeta, 16)) FAIL(3);
-    orc_challenger_observe(&ch, ys, 4 * n_open);
-    orc_challenger_sample_ext(&ch, t4);
-    if (memcmp(t4, proof->gamma, 16)) FAIL(4);
-    for (uint32_t i = 0; i < proof->n_fri_layers; i++) {
-        orc_challenger_observe(&ch, proof->fri_roots[i], 8);
-        orc_challenger_sample_ext(&ch, t4);
-        if (memcmp(t4, proof->fri_betas[i], 16)) FAIL(5);
-    }
-    /* the final polynomial has one coefficient: both evaluations of the last layer must be that constant */
-    if (memcmp(proof->final_poly[0], proof->final_poly[1], 16)) FAIL(15);
-    orc_challenger_observe(&ch, proof->final_poly[0], 4);
-    {
-        const uint32_t mask = proof->pow_bits >= 31 ? 0x7fffffffu : ((1u << proof->pow_bits) - 1);
-        if (proof->pow_witness >= BB_P) FAIL(6);
-        orc_challenger_observe(&ch, &proof->pow_witness, 1);
-        if (orc_challenger_sample(&ch) & mask) FAIL(6);
-    }
-
-    const bb4_t zeta = ld4(proof->zeta), gamma = ld4(proof->gamma), alpha = ld4(proof->alpha);
-    const bb4_t zeta_next = bb4_scale(zeta, bb_root_of_unity(log_n));
-    const uint32_t* ys_main = ys;
-    const uint32_t* ys_perm = ys + 4 * width;
-    const uint32_t* ys_perm_next = ys + 4 * (width + wp);
-    const uint32_t* ys_q = ys + 4 * (width + 2 * wp);
-
-    /* 2. constraint identity at zeta (only meaningful for a satisfying trace) */
-    if (check_constraints) {
-        bb4_t acc = bb4_from_base(0);
-        for (size_t k = 0; k < air->n_constraints; k++) {
-            acc = bb4_mul(acc, alpha);
-            acc = bb4_add(acc, eval_ext(air->bc + air->spans[k].off, air->spans[k].len, ys_main));
-        }
-        if (air->n_ints)
-            acc = orc_logup_fold_at_point(acc, alpha, ys_main, ys_perm, ys_perm_next, log_n, zeta, air->ibc, air->ispans, air->ints, air->n_ints,
-                                          chunk_start, n_chunks, ld4(proof->logup_alpha), proof->logup_beta, ld4(proof->cumulative_sum));
-        bb4_t zn = bb4_pow(zeta, n);
-        uint32_t gn = bb_pow(BB_GENERATOR, n);
-        /* Q(zeta) = sum_b (zeta^N - g^N (-1)^(1-b)) / (2 g^N (-1)^b) * Q_b(zeta),  Q_b = sum_l x^l-basis limb l of chunk b */
-        bb4_t q = bb4_from_base(0);
-        for (int b = 0; b < 2; b++) {
-            uint32_t sgn_b = b ? BB_P - 1 : 1, sgn_nb = b ? 1 : BB_P - 1;
-            bb4_t num = zn;
-            num.c[0] = bb_sub(num.c[0], bb_mul(gn, sgn_nb));
-            uint32_t den = bb_inv(bb_mul(2, bb_mul(gn, sgn_b)));
-            bb4_t qb = bb4_from_base(0);
-            for (int l = 0; l < 4; l++) {
-                bb4_t e = bb4_from_base(0);
-                e.c[l] = 1;                                             /* basis element x^l of Ext4 */
-                qb = bb4_add(qb, bb4_mul(e, ld4(ys_q + 4 * (4 * b + l))));
-            }
-            q = bb4_add(q, bb4_mul(bb4_scale(num, den), qb));
-        }
-        bb4_t zh = zn;
-        zh.c[0] = bb_sub(zh.c[0], 1);
-        if (!eq4(acc, bb4_mul(zh, q))) FAIL(16);
-    }
-
-    /* 3. queries */
-    const size_t wpq = orc_query_words(log_n, width, wp);
-    gp = (bb4_t*)malloc(n_open * sizeof(bb4_t));
-    bb4_t cur = bb4_from_base(1), ysum0 = bb4_from_base(0), ysum1 = bb4_from_base(0);
-    for (size_t j = 0; j < n_open; j++) {
-        gp[j] = cur;
-        const int next_group = j >= width + wp && j < width + 2 * wp;
-        if (next_group) ysum1 = bb4_add(ysum1, bb4_mul(cur, ld4(ys + 4 * j)));
-        else ysum0 = bb4_add(ysum0, bb4_mul(cur, ld4(ys + 4 * j)));
-        cur = bb4_mul(cur, gamma);
-    }
-    const uint32_t two_inv = bb_inv(2);
-    for (size_t qi = 0; qi < n_queries && !rc; qi++) {
-        const uint32_t* o = queries + qi * wpq;
-        const size_t r = o[0];
-        if (r != (orc_challenger_sample(&ch) & (((size_t)1 << log_m) - 1))) { rc = 7; break; }
-        const uint32_t* trow = o + 1;
-        const uint32_t* tpath = trow + width;
-        const uint32_t* prow = tpath + 8 * log_m;
-        const uint32_t* ppath = prow + wp;
-        const uint32_t* qrow = wp ? ppath + 8 * log_m : prow;
-        const uint32_t* qpath = qrow + 8;
-        const uint32_t* fr = qpath + 8 * log_m;
-        uint32_t leaf[8];
-        orc_hash_row(trow, width, leaf);
-        if (!check_path(leaf, r, tpath, log_m, proof->trace_root)) { rc = 8; break; }
-        if (wp) {
-            orc_hash_row(prow, wp, leaf);
-            if (!check_path(leaf, r, ppath, log_m, proof->perm_root)) { rc = 9; break; }
-        }
-        orc_hash_row(qrow, 8, leaf);
-        if (!check_path(leaf, r, qpath, log_m, proof->quotient_root)) { rc = 10; break; }
-        bb4_t a0 = bb4_from_base(0), a1 = bb4_from_base(0);
-        for (size_t j = 0; j < width; j++) a0 = bb4_add(a0, bb4_scale(gp[j], trow[j]));
-        for (size_t j = 0; j < wp; j++) {
-            a0 = bb4_add(a0, bb4_scale(gp[width + j], prow[j]));
-            a1 = bb4_add(a1, bb4_scale(gp[width + wp + j], prow[j]));
-        }
-        for (size_t j = 0; j < 8; j++) a0 = bb4_add(a0, bb4_scale(gp[width + 2 * wp + j], qrow[j]));
-        a0 = bb4_sub(a0, ysum0);
-        a1 = bb4_sub(a1, ysum1);
-        uint32_t x = bb_mul(BB_GENERATOR, bb_pow(bb_root_of_unity(log_m), bitrev32((uint32_t)r, log_m)));
-        bb4_t d0 = bb4_sub(bb4_from_base(x), zeta), d1 = bb4_sub(bb4_from_base(x), zeta_next);
-        bb4_t val = bb4_mul(a0, bb4_inv(d0));
-        if (wp) val = bb4_add(val, bb4_mul(a1, bb4_inv(d1)));
-        size_t idx = r;
-        uint32_t shift = BB_GENERATOR;
-        for (unsigned i = 0; i < log_n; i++) {
-            const unsigned log_len = log_m - i, log_h = log_len - 1;
-            const uint32_t* pair = fr;
-            const uint32_t* path = fr + 8;
-            fr += 8 + 8 * log_h;
-            bb4_t lo = ld4(pair), hi = ld4(pair + 4);
-            if (!eq4((idx & 1) ? hi : lo, val)) { rc = i == 0 ? 11 : 13; break; }
-            const size_t j = idx >> 1;
-            orc_hash_row(pair, 8, leaf);
-            if (!check_path(leaf, j, path, log_h, proof->fri_roots[i])) { rc = 12; break; }
-            uint32_t xj = bb_mul(shift, bb_pow(bb_root_of_unity(log_len), bitrev32((uint32_t)j, log_h)));
-            bb4_t beta = ld4(proof->fri_betas[i]);
-            bb4_t s = bb4_scale(bb4_add(lo, hi), two_inv);
-            bb4_t df = bb4_scale(bb4_sub(lo, hi), bb_mul(two_inv, bb_inv(xj)));
-            val = bb4_add(s, bb4_mul(beta, df));
-            idx = j;
-            shift = bb_mul(shift, shift);
-        }
-        if (!rc && !eq4(val, ld4(proof->final_poly[idx]))) rc = 14;
-    }
-done:
-    free(gp);
-    free(chunk_start);
-    return rc;
-#undef FAIL
-}
-
-/* =====================================================================================================================
- * verifier of the multi-chip segment proof (orc_prove_chips): one transcript, mixed-height MMCS openings, one FRI instance with
- * per-height injection of the reduced openings. */
+/* one opened row of a matrix of height 2^log_h; a mixed-height MMCS path is checked as prove.c commits it */
 typedef struct { const uint32_t* row; size_t width; unsigned log_h; } mv_mat_t;
 
 static void hash_opened(const mv_mat_t* ms, size_t n, unsigned log_h, uint32_t digest[8]) {

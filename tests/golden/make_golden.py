@@ -12,8 +12,10 @@ reference-derived fixtures and the oracle for the generated vectors):  python te
   fixture_stats.json               sizes/degree histograms of the big reference fixtures (keccak/sha256/ecrecover ...)
   oracle_kat.json                  known-answer vectors produced BY THE ORACLE (Poseidon2, sponge, compress, challenger,
                                    small LDE / fold) -- regression pins for oracle and GPU alike
-  segment_2p8_w12.json             a whole-segment proof produced by the oracle
+  segment_2p8_w12.json             a whole-segment proof produced by the oracle (orc.prove: the one-chip proof of orc_prove_chips)
   segment_logup_2p7.json           the same with bus interactions (LogUp phase, transcript v2): proof + digests of the opened values / queries
+  segment_shapes.json              the same for 2-, 4- and 32-row traces, each with constraints and interactions, constraints only and
+                                   interactions only: first written by a dedicated single-chip prover, so it pins the one-chip proof to it
   stage0_subs.json.gz              instruction opcodes + per-instruction substitution tables (`block`, `subs` sections) of
                                    single_div_nondet, wasm_register_reuse and keccak_apc_pre_opt (677 instructions, 27 521 cells): the
                                    REAL stage-0 gather pattern (the machines of the big fixture are not committed: 28 627 constraints)
@@ -126,6 +128,7 @@ def main():
 
     chips_fixture("chips_mixed.json", [[6, 12, 3, 7], [4, 9, 2, 0], [3, 10, 0, 3]], seed=5, n_queries=6, pow_bits=5)
     chips_fixture("chips_tiny.json", [[1, 6, 2, 3], [2, 7, 0, 4], [5, 9, 3, 2], [1, 5, 1, 0]], seed=7, n_queries=8, pow_bits=4)
+    segment_shapes_fixture("segment_shapes.json", seed=11, n_queries=6, pow_bits=3)
 
 
 def chips_fixture(name, spec, seed, n_queries, pow_bits):
@@ -136,6 +139,21 @@ def chips_fixture(name, spec, seed, n_queries, pow_bits):
     chips = chips_for(g["spec"], g["seed"])
     proof, cs, ys, q = orc.prove_chips(chips, n_queries=g["n_queries"], pow_bits=g["pow_bits"])
     g.update(proof=proof, cumsums=cs.tolist(), ys_sha256=sha(ys), queries_sha256=sha(q))
+    dump(name, g)
+
+
+def segment_shapes_fixture(name, seed, n_queries, pow_bits):
+    """single-segment proofs (orc.prove) of 2-, 4- and 32-row traces, each for an AIR with constraints and interactions, one with
+    constraints only and one with interactions only: proof fields, digests of the opened values and query words"""
+    import hashlib
+    sha = lambda a: hashlib.sha256(np.ascontiguousarray(a, dtype=np.uint32).tobytes()).hexdigest()
+    g = {"seed": seed, "n_queries": n_queries, "pow_bits": pow_bits, "cases": []}
+    for log_n in (1, 2, 5):
+        for width, ncons, nints in ((10, 3, 4), (9, 4, 0), (8, 0, 5)):
+            spec = [log_n, width, ncons, nints]
+            trace, bc, spans, bus = chips_for([spec], seed)[0]
+            proof, ys, q, _ = orc.prove(trace, bc, spans, bus, n_queries=n_queries, pow_bits=pow_bits)
+            g["cases"].append({"spec": spec, "proof": proof, "ys_sha256": sha(ys), "queries_sha256": sha(q)})
     dump(name, g)
 
 

@@ -35,16 +35,26 @@ def test_mixed_heights_with_and_without_interactions_verify(orc):
         assert p2 == proof and (cs2 == cs).all() and (ys2 == ys).all() and (q2 == q).all()
 
 
-def test_one_chip_reduces_to_the_same_commitments_as_the_single_chip_prover(orc):
-    chips = _chips([(5, 11, 4, 6)], seed=2)
-    proof, cs, ys, q = orc.prove_chips(chips, n_queries=4, pow_bits=3)
-    trace, bc, spans, bus = chips[0]
-    single, ys1, q1, _ = orc.prove(trace, bc, spans, bus, n_queries=4, pow_bits=3)
-    # with one chip the MMCS trees degenerate to plain Merkle trees and the transcript is the same: identical proof material
-    assert proof["main_root"] == single["trace_root"] and proof["perm_root"] == single["perm_root"]
-    assert proof["quotient_root"] == single["quotient_root"] and proof["fri_roots"] == single["fri_roots"]
-    assert proof["pow_witness"] == single["pow_witness"] and (ys == ys1).all() and (q == q1).all()
-    assert cs[0].tolist() == single["cumulative_sum"]
+def test_one_chip_proofs_reproduce_the_single_segment_fixture(orc):
+    """tests/golden/segment_shapes.json pins single-segment proofs of 2-, 4- and 32-row traces (AIRs with constraints and
+    interactions, constraints only, interactions only) as a dedicated single-chip prover wrote them; the one-chip proof must be
+    the same proof, opened values and query words, in slow and in fast mode"""
+    import hashlib
+    import json
+    import os
+    import sys
+    golden = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+    sys.path.insert(0, golden)
+    from make_golden import chips_for
+    sha = lambda a: hashlib.sha256(np.ascontiguousarray(a, dtype=np.uint32).tobytes()).hexdigest()
+    g = json.load(open(os.path.join(golden, "segment_shapes.json")))
+    assert len(g["cases"]) == 9
+    for case in g["cases"]:
+        trace, bc, spans, bus = chips_for([case["spec"]], g["seed"])[0]
+        for fast in ([False, True] if orc.fast_available() else [False]):
+            proof, ys, q, _ = orc.prove(trace, bc, spans, bus, n_queries=g["n_queries"], pow_bits=g["pow_bits"], fast=fast)
+            assert proof == case["proof"] and sha(ys) == case["ys_sha256"] and sha(q) == case["queries_sha256"], (case["spec"], fast)
+        assert orc.verify_segment(bc, spans, case["spec"][0], trace.shape[0], proof, ys, q, bus=bus) == 0
 
 
 def test_satisfying_and_unsatisfying_traces(orc):
@@ -108,8 +118,9 @@ def test_random_chip_mixes_verify_and_bind_every_opened_value(orc):
 
 
 def test_committed_fixtures_are_reproduced(orc):
-    """tests/golden/segment_logup_2p7.json, chips_mixed.json and chips_tiny.json (written by tests/golden/make_golden.py): regression pins of transcript
-    v2 with the LogUp phase and of the multi-chip transcript -- proof fields exactly, opened values / query openings by digest"""
+    """tests/golden/segment_2p8_w12.json, segment_logup_2p7.json, chips_mixed.json and chips_tiny.json (written by
+    tests/golden/make_golden.py): regression pins of transcript v2 without and with the LogUp phase and of the multi-chip
+    transcript -- proof fields exactly, opened values / query openings by digest"""
     import hashlib
     import json
     import os
@@ -119,6 +130,12 @@ def test_committed_fixtures_are_reproduced(orc):
     sys.path.insert(0, golden)
     from make_golden import chips_for
     sha = lambda a: hashlib.sha256(np.ascontiguousarray(a, dtype=np.uint32).tobytes()).hexdigest()
+    g = json.load(open(os.path.join(golden, "segment_2p8_w12.json")))
+    mach = M.synthetic_machine(g["width"], g["n_constraints"], seed=g["seed"])
+    bc, spans = M.compile_constraints(mach)
+    trace = rand_field(np.random.default_rng(g["trace_seed"]), (mach.width, 1 << g["log_n"]))
+    for fast in ([False, True] if orc.fast_available() else [False]):
+        assert orc.prove_segment(trace, bc, spans, fast=fast)[0] == g["proof"]
     g = json.load(open(os.path.join(golden, "segment_logup_2p7.json")))
     base = M.synthetic_machine(g["width"], g["n_constraints"], seed=g["seed"])
     mach = M.SymbolicMachine(base.constraints, M.synthetic_bus(base, g["n_interactions"], g["bus_seed"], g["quadratic_every"]))
