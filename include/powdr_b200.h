@@ -194,6 +194,24 @@ int pb_chips_sizes(const pb_chip_t* chips, size_t n_chips, size_t* n_opened, siz
 /* queries ([n_queries][words_per_query], may be NULL) and opened values ([n_opened][4], may be NULL) of the last pb_prove_chips */
 int pb_query_chips(pb_ctx_t* ctx, uint32_t* h_queries, size_t queries_capacity_words, uint32_t* h_ys, size_t ys_capacity_words);
 
+/* ---- device memory of the single-GPU provers (pb_prove_segment, pb_prove_chips) ---------------------------------------------
+ * A proof whose footprint fits the budget keeps every committed matrix resident (the LDEs of the traces and permutation traces).  One
+ * that does not is proved in B = 2^log_blocks row blocks, 2 <= B <= 16: the chips of its tallest LDE heights keep their coefficients
+ * (the permutation trace becomes its coefficients in place) and one row block of each LDE, which every phase that reads the LDE (the
+ * main and permutation commitments, the quotient, the reduced opening, the query phase) recomputes block by block.  The proof is the
+ * same, word for word.  A height is blocked for all of its chips or none, and only if log_n >= log_blocks + 3.  The prover takes the
+ * resident path when it fits, else the smallest B and, at that B, the fewest blocked heights (tallest first) that fit; if nothing fits
+ * it returns cudaErrorMemoryAllocation (2) before launching anything.  A host-resident trace (pb_prove_segment without
+ * PB_TRACE_ON_DEVICE) is copied whole to the device first and counts in the footprint. */
+/* the budget: by default the device's free memory at the call plus what the context's proof workspaces hold; `bytes` lowers it, 0
+ * restores the default */
+int pb_ctx_set_memory_budget(pb_ctx_t* ctx, size_t bytes);
+/* log2 of the row blocks of the last pb_prove_segment / pb_prove_chips of the context: 0 for the resident path */
+int pb_last_row_blocks(pb_ctx_t* ctx, uint32_t* log_blocks);
+/* the bytes the choice above counts for chips of these heights, widths and permutation widths (pb_air_perm_width) with device-resident
+ * traces (not counted), every height with log_n >= log_blocks + 3 in 2^log_blocks row blocks (0: resident); needs no device */
+int pb_footprint_bytes(const size_t* log_n, const size_t* width, const size_t* perm_width, size_t n_chips, uint32_t log_blocks, size_t* bytes);
+
 /* ---- one segment across G = 2^g GPUs, one process (and one pb_ctx) per GPU: SURVEY.md §8e ----
  * The trace is column-sharded on input (rank r holds columns pb_shard_columns(width, G, r)), the LDE and everything after it
  * is row-sharded (rank r holds rows [r*2N/G, (r+1)*2N/G) of the bit-reversed LDE for ALL columns); one all-to-all of folded

@@ -18,7 +18,7 @@ EXPORTS = [
     "pb_merkle_commit_rows8", "pb_poseidon2_permute", "pb_fri_fold", "pb_eval_at_point", "pb_deep_quotient", "pb_prove_segment", "pb_query_words", "pb_query_segment", "pb_last_openings", "pb_last_stage_ms",
     "pb_ctx_set_fri_params", "pb_air_set_interactions", "pb_air_perm_width", "pb_air_logup_compile_only", "pb_allgather_caps", "pb_bus_compile", "pb_bus_free", "pb_bus_apply",
     "pb_shard_columns", "pb_lde_shard", "pb_prove_segment_sharded", "pb_query_segment_sharded", "pb_prove_chips", "pb_chips_sizes", "pb_query_chips", "pb_host_poseidon2_permute",
-    "pb_prove_chips_sharded", "pb_query_chips_sharded",
+    "pb_prove_chips_sharded", "pb_query_chips_sharded", "pb_ctx_set_memory_budget", "pb_last_row_blocks", "pb_footprint_bytes",
     "pb_launch_count", "pb_leaf_kernel_profile", "_apc_tracegen", "_apc_apply_derived_expr", "_apc_apply_bus",
 ]
 
@@ -95,6 +95,16 @@ STAGES = ("h2d", "lde", "merkle", "logup_gen", "logup_commit", "quotient", "qlde
 
 
 _lib = None
+
+
+def footprint_bytes(chips, log_blocks=0):
+    """chips: [(log_n, width, perm_width)] -> the device bytes pb_footprint_bytes counts for a proof of them in 2^log_blocks row blocks"""
+    lib = load_library()
+    k = len(chips)
+    ln, w, wp = [(C.c_size_t * k)(*[int(c[i]) for c in chips]) for i in range(3)]
+    out = C.c_size_t()
+    _chk(lib.pb_footprint_bytes(ln, w, wp, C.c_size_t(k), C.c_uint32(log_blocks), C.byref(out)), "pb_footprint_bytes")
+    return int(out.value)
 
 
 def load_library(path=None):
@@ -371,6 +381,16 @@ class Context:
                                              C.c_size_t(q.size if q is not None else 0), ys.ctypes.data_as(C.c_void_p), C.c_size_t(ys.size)),
              "pb_query_chips_sharded")
         return ys, q
+
+    def set_memory_budget(self, nbytes):
+        """device memory the single-GPU provers may use (0: free memory at the call + what the context holds)"""
+        _chk(self.lib.pb_ctx_set_memory_budget(self.h, C.c_size_t(int(nbytes))), "pb_ctx_set_memory_budget")
+
+    def last_row_blocks(self):
+        """log2 of the row blocks of the last prove_segment / prove_chips (0: resident)"""
+        lb = C.c_uint32()
+        _chk(self.lib.pb_last_row_blocks(self.h, C.byref(lb)), "pb_last_row_blocks")
+        return int(lb.value)
 
     def last_stage_ms(self):
         ms = (C.c_float * len(STAGES))()

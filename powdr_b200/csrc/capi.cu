@@ -109,6 +109,8 @@ struct DevBuf {
         cap = n;
         return 0;
     }
+    void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
+    int fit(size_t n) { if (cap > n) release(); return ensure(n); }      // exactly n: a larger buffer of an earlier proof is freed
 };
 
 __global__ void to_monty_kernel(uint32_t* a, size_t n) {
@@ -147,12 +149,13 @@ struct pb_bus {
 
 // one chip of a proof (chips.inl): its matrices stay resident until the query phase.  pb_prove_segment uses slot 0.  The sharded provers
 // (shard_api.inl) hold their row blocks here; their `perm` is [my trace rows x the padded permutation columns | row sums | my permutation
-// columns, whole].
+// columns, whole].  A chip proved in 2^lb row blocks (lb > 0, single GPU) keeps its main coefficients in `coef` and its permutation
+// coefficients in `perm`; `lde` and `perm_lde` hold one row block, recomputed by each phase that reads it (rowblock.inl).
 struct McChip {
-    size_t log_n = 0, width = 0, wp = 0, n_chunks = 0, e_main = 0, e_perm = 0, e_q = 0;
+    size_t log_n = 0, width = 0, wp = 0, n_chunks = 0, e_main = 0, e_perm = 0, e_q = 0, lb = 0;
     const pb_air* air = nullptr;
     const uint32_t* d_trace = nullptr;
-    DevBuf<uint32_t> lde, perm, perm_lde, qnat, qlde;
+    DevBuf<uint32_t> lde, perm, perm_lde, qnat, qlde, coef;
     bb::E4 cumsum = {{0u, 0u, 0u, 0u}};
 };
 
@@ -184,6 +187,8 @@ struct pb_ctx {
     DevBuf<uint32_t> ws_rowsum, ws_scan_tot, ws_lu_raw, ws_lu_s, ws_pow;   // LogUp phase + PoW
     DevBuf<uint32_t> ws_mc_dig;           // digests of the shorter height groups until the tree reaches their level
     uint32_t n_queries = 100, pow_bits = 16;
+    size_t mem_budget = 0;                // pb_ctx_set_memory_budget (0: free device memory + what the proof workspaces hold)
+    uint32_t last_lb = 0;                 // log2 of the row blocks of the last single-GPU proof (0: resident)
     DevBuf<uint32_t> ws_fri_ch, ws_fri_log;  // device challenger state and the (root, beta) log of the FRI commit phase
     DevBuf<uint32_t> ws_sh_qall;             // every rank's share of the query openings
     DevBuf<shard::Xfer> ws_sh_tab;           // chip table of the batched exchanges
@@ -897,6 +902,7 @@ static int fri_commit_phase(pb_ctx* ctx, Challenger& ch, uint32_t layer0, size_t
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
+static int eval_weighted_m(pb_ctx* ctx, const uint32_t* d_mat, size_t N, size_t width, bb::E4 pref, uint32_t* d_ys);
 // openings: y_k = f_k(zeta) for columns given as evaluations over shift*H (natural order); d_ys: [width][4] Montgomery
 static int eval_at_point_m(pb_ctx* ctx, const uint32_t* d_mat, size_t log_n, size_t width, uint32_t shift_m, bb::E4 zeta_m, uint32_t* d_ys) {
     const size_t N = (size_t)1 << log_n;
@@ -911,10 +917,14 @@ static int eval_at_point_m(pb_ctx* ctx, const uint32_t* d_mat, size_t log_n, siz
     for (size_t i = 0; i < log_n; i++) zn = bb::e4_mul(zn, zn);
     zn.c[0] = bb::sub(zn.c[0], bb::R1);
     const bb::E4 pref = bb::e4_scale(zn, bb::inv(h_to_m((uint32_t)(N % bb::P))));
+    return eval_weighted_m(ctx, d_mat, N, width, pref, d_ys);
+}
+
+// y_k = pref * sum_i mat[k][i] * ws_w[i]
+static int eval_weighted_m(pb_ctx* ctx, const uint32_t* d_mat, size_t N, size_t width, bb::E4 pref, uint32_t* d_ys) {
     const uint32_t rows_per_cta = (uint32_t)std::max<size_t>(deep::EV_THREADS, std::min<size_t>(N, (size_t)1 << 15));
     const uint32_t splits = (uint32_t)((N + rows_per_cta - 1) / rows_per_cta);
-    rc = ctx->ws_part.ensure(width * splits);
-    if (rc) return rc;
+    RC(ctx->ws_part.ensure(width * splits));
     dim3 grid((unsigned)((width + deep::EV_COLS - 1) / deep::EV_COLS), splits);
     deep::eval_partial_kernel<<<grid, deep::EV_THREADS, 0, ctx->stream>>>(d_mat, N, (uint32_t)width, ctx->ws_w.p, ctx->ws_part.p, rows_per_cta);
     LAUNCHED(ctx);
@@ -1019,6 +1029,20 @@ static int deep_quotient_groups_m(pb_ctx* ctx, const std::vector<const uint32_t*
     CK(cudaGetLastError());
     return 0;
 }
+// the same values for columns given as coefficients in bit-reversed slots, scaled as the inverse LDE passes leave them (the true
+// coefficients): y_k = sum_j coef[k][j] * z^bitrev(j)
+static int eval_coefs_at_point_m(pb_ctx* ctx, const uint32_t* d_coef, size_t log_n, size_t width, bb::E4 z, uint32_t* d_ys) {
+    const size_t N = (size_t)1 << log_n;
+    if (width == 0) return 0;
+    RC(ctx->ws_w.ensure(N));
+    deep::ZPow2 zp{};
+    bb::E4 x = z;
+    for (size_t k = 0; k < log_n; k++) { zp.p[k] = x; x = bb::e4_mul(x, x); }
+    deep::monomial_weights_kernel<<<(unsigned)((N + 255) / 256), 256, 0, ctx->stream>>>(ctx->ws_w.p, (int)log_n, zp);
+    LAUNCHED(ctx);
+    return eval_weighted_m(ctx, d_coef, N, width, bb::E4{{bb::R1, 0u, 0u, 0u}}, d_ys);
+}
+
 int pb_eval_at_point(pb_ctx_t* ctx, const uint32_t* d_mat, size_t log_n, size_t width, uint32_t shift, const uint32_t zeta[4], uint32_t* d_ys) {
     if (!ctx || !d_mat || !zeta || !d_ys) return PB_ERR_INVALID_ARG;
     if (log_n < 1 || log_n > 27 || shift == 0 || shift >= bb::P) return PB_ERR_UNSUPPORTED;
@@ -1150,5 +1174,6 @@ int pb_bus_apply(pb_ctx_t* ctx, const pb_bus_t* b, const uint32_t* d_trace, size
 }
 
 #include "shard_api.inl"
+#include "rowblock.inl"
 
 }  // extern "C"

@@ -38,6 +38,19 @@ __global__ void __launch_bounds__(256) bary_weights_kernel(uint4* __restrict__ w
     w[i] = make_uint4(r.c[0], r.c[1], r.c[2], r.c[3]);
 }
 
+// monomial weights for coefficients in bit-reversed slots (what the inverse LDE passes leave):  w_j = z^bitrev(j), so that
+// sum_j coef_j * w_j = f(z).  zp[k] = z^(2^k); bit i of j contributes zp[log_n - 1 - i].
+struct ZPow2 { bb::E4 p[24]; };
+__global__ void __launch_bounds__(256) monomial_weights_kernel(uint4* __restrict__ w, int log_n, ZPow2 zp) {
+    const size_t j = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= ((size_t)1 << log_n)) return;
+    bb::E4 r = {{bb::R1, 0u, 0u, 0u}};
+#pragma unroll
+    for (int k = 0; k < 24; k++)          // unrolled: zp stays in the parameter space
+        if (k < log_n && ((j >> (log_n - 1 - k)) & 1)) r = bb::e4_mul(r, zp.p[k]);
+    w[j] = make_uint4(r.c[0], r.c[1], r.c[2], r.c[3]);
+}
+
 // 96-bit accumulator a += f * g.  ptxas turns the carry chain into IMAD.WIDE.U32 with a carry-out predicate and folds two
 // carries into one IADD3.X, i.e. 1 multiplier-pipe + 0.5 ALU instruction per MAC.
 struct Acc96 { uint32_t w0, w1, w2; };
