@@ -28,6 +28,7 @@ extern "C" {
 #define PB_ERR_NO_DEVICE (-5)
 #define PB_ERR_COMM (-6)          /* a caller-supplied collective (pb_comm_t) reported failure */
 #define PB_ERR_INTERNAL (-7)      /* a self-check failed (the host replay of the device-driven FRI transcript disagreed): a bug */
+#define PB_ERR_REJECTED (-8)      /* pb_verify_*: the proof is not accepted; *reason says which check failed */
 
 #define PB_BABYBEAR_P 2013265921u
 #define PB_DIGEST_WORDS 8
@@ -305,6 +306,51 @@ int pb_air_perm_width(const pb_air_t* air, size_t* perm_width);
  * all_caps[r*8 .. r*8+8) = rank r's local_cap, through the caller's pb_comm_t (device pointers; no NCCL is linked here, which is
  * also why pb_ctx_create takes no ncclComm_t: the collectives are callbacks so that the same library serves NCCL, MPI or tests) */
 int pb_allgather_caps(pb_ctx_t* ctx, const pb_comm_t* comm, const uint32_t* d_local_cap, uint32_t* d_all_caps);
+
+/* ---- verifying a proof on the host: no device, no CUDA context, no NVRTC ----------------------------------------------------------
+ * Where the reference checks its own prover, verify_app_proof on the CPU engine (the reference's openvm-riscv/src/lib.rs:337-341), and
+ * what a prover service calls before it publishes a proof.  The key of an AIR holds what the verifier reads of it: the constraints and
+ * the bus interactions in the arrays pb_air_compile and pb_air_set_interactions take, validated by the same code (PB_ERR_BAD_BYTECODE,
+ * PB_ERR_STACK_DEPTH, PB_ERR_UNSUPPORTED for an interaction above the degree bound, exactly where those return them).  n_interactions = 0:
+ * an AIR without interactions (the bus arrays are then not read). */
+typedef struct pb_vk pb_vk_t;
+int pb_vk_create(const uint32_t* bytecode, size_t n_words, const pb_expr_span_t* constraints, size_t n_constraints, uint32_t width,
+                 const uint32_t* bus_bytecode, size_t bus_words, const ExprSpan* arg_spans, size_t n_arg_spans,
+                 const DevInteraction* interactions, size_t n_interactions, pb_vk_t** out);
+int pb_vk_free(pb_vk_t* vk);
+/* one chip of the proof: its key and log2 of its trace height (1..24) */
+typedef struct { const pb_vk_t* vk; size_t log_n; } pb_verify_chip_t;
+/* the verifier's security parameters, which the proof must match (n_queries 1..65536, pow_bits 0..30), and its Poseidon2 instance
+ * (canonical values as for pb_ctx_set_poseidon2; all three NULL: the default of include/pb_poseidon2_constants.h) */
+typedef struct {
+    uint32_t n_queries, pow_bits;
+    const uint32_t (*rc_ext)[16];
+    const uint32_t* rc_int;
+    const uint32_t* diag_m1;
+} pb_verify_params_t;
+/* pb_verify_chips checks a proof of pb_prove_chips / pb_prove_chips_sharded, given what those and pb_query_chips(_sharded) return:
+ * h_cumsums [n_chips][4], h_ys [n_opened][4] and h_queries [n_queries][words_per_query], ys_words and queries_words being the lengths
+ * of the last two.  It checks, in this order, with *reason (may be NULL) set to the first failure:
+ *   20 proof shape: a chip height outside 1..24, or n_chips, log_max, n_fri_layers, final_len not following from the chip heights;
+ *   21 the proof's n_queries or pow_bits differ from params;
+ *   then the lengths, which must be what pb_chips_sizes gives for these chips (else PB_ERR_INVALID_ARG): no buffer is read before;
+ *   20 also: a nonzero cumulative sum for a chip without interactions (it has none, and a caller's bus balance sums every slot);
+ *   22 a word of h_ys, h_cumsums, the query openings (index aside), a digest, final_poly or pow_witness is not canonical (>= p);
+ *   then it replays the transcript of DESIGN.md §3 / §3b:
+ *   1 LogUp challenges, 2 alpha, 3 zeta, 4 gamma, 5 a FRI beta, 15 final polynomial not constant, 6 proof of work;
+ *   16 per chip the constraint identity at zeta: Horner_alpha(AIR constraints, LogUp chunk and phi constraints) = Z_H(zeta) * Q(zeta);
+ *   per query: 7 index, 8 / 9 / 10 main / permutation / quotient MMCS opening, 11 reduced opening != FRI layer 0, 12 FRI path,
+ *   13 fold, 14 final value.
+ * -> 0 accepted, PB_ERR_REJECTED, or PB_ERR_INVALID_ARG (NULL pointers, a chip without a key, n_chips = 0, mismatched lengths, bad
+ * params).  The bus balance (the cumulative sums of ALL chips of a segment add up to zero) is the caller's check: a proof of the APC
+ * chips alone does not contain the chips that balance their buses.  Pure host code: thread-safe, no CUDA call. */
+int pb_verify_chips(const pb_verify_chip_t* chips, size_t n_chips, const pb_verify_params_t* params, const pb_chips_proof_t* proof,
+                    const uint32_t* h_cumsums, const uint32_t* h_ys, size_t ys_words, const uint32_t* h_queries, size_t queries_words,
+                    int* reason);
+/* a proof of pb_prove_segment / pb_prove_segment_sharded with pb_query_segment(_sharded) and pb_last_openings: the one-chip case of
+ * pb_verify_chips, its cumulative_sum being h_cumsums (a perm_width other than the key's is reason 20, after the argument checks) */
+int pb_verify_segment(const pb_vk_t* vk, size_t log_n, const pb_verify_params_t* params, const pb_segment_proof_t* proof,
+                      const uint32_t* h_ys, size_t ys_words, const uint32_t* h_queries, size_t queries_words, int* reason);
 
 int _apc_tracegen(uint32_t* d_output, size_t output_height, const OriginalAir* d_original_airs, const Subst* d_subs,
                   size_t n_subs, int num_apc_calls);

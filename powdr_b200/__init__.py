@@ -2,10 +2,11 @@
 
 The product is the sm_90a shared library behind include/powdr_b200.h; this package is the thin host-side mirror of the
 reference's Rust call sites (machine JSON -> bytecode, launch wrappers, segment proving).  There is no CPU fallback:
-importing works anywhere, but every compute call needs the CUDA library and a GPU.
+importing works anywhere, but every proving call needs the CUDA library and a GPU.  The verifier (VerifyingKey, verify_chips,
+verify_segment) is host code in the same library and needs no GPU.
 """
-from .capi import Context, Air, load_library, LibraryMissing, P  # noqa: F401
+from .capi import Context, Air, VerifyingKey, verify_chips, verify_segment, load_library, LibraryMissing, P  # noqa: F401
 from .machine import SymbolicMachine, compile_constraints, compile_derived, compile_bus  # noqa: F401
 
-__all__ = ["Context", "Air", "load_library", "LibraryMissing", "P", "SymbolicMachine", "compile_constraints",
+__all__ = ["Context", "Air", "VerifyingKey", "verify_chips", "verify_segment", "load_library", "LibraryMissing", "P", "SymbolicMachine", "compile_constraints",
            "compile_derived", "compile_bus"]

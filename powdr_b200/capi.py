@@ -20,7 +20,10 @@ EXPORTS = [
     "pb_shard_columns", "pb_lde_shard", "pb_prove_segment_sharded", "pb_query_segment_sharded", "pb_prove_chips", "pb_chips_sizes", "pb_query_chips", "pb_host_poseidon2_permute",
     "pb_prove_chips_sharded", "pb_query_chips_sharded", "pb_ctx_set_memory_budget", "pb_last_row_blocks", "pb_footprint_bytes",
     "pb_launch_count", "pb_leaf_kernel_profile", "_apc_tracegen", "_apc_apply_derived_expr", "_apc_apply_bus",
+    "pb_vk_create", "pb_vk_free", "pb_verify_chips", "pb_verify_segment",
 ]
+PB_ERR_INVALID_ARG = -1
+PB_ERR_REJECTED = -8
 
 
 class LibraryMissing(RuntimeError):
@@ -73,6 +76,19 @@ class SegmentProof(C.Structure):
         d["final_poly"] = [list(self.final_poly[i]) for i in range(self.final_len)]
         return d
 
+    @classmethod
+    def from_dict(cls, d):
+        """the struct of an as_dict() result"""
+        p = cls()
+        for k in cls.VEC:
+            getattr(p, k)[:] = [int(v) for v in d[k]]
+        for k in cls.SCALAR:
+            setattr(p, k, int(d[k]))
+        for name, rows in (("fri_roots", d["fri_roots"]), ("fri_betas", d["fri_betas"]), ("final_poly", d["final_poly"])):
+            for i, row in enumerate(rows):
+                getattr(p, name)[i][:] = [int(v) for v in row]
+        return p
+
 
 class Chip(C.Structure):
     """pb_chip_t"""
@@ -89,6 +105,17 @@ class ChipsProof(C.Structure):
     VEC = ("main_root", "perm_root", "quotient_root", "logup_alpha", "logup_beta", "alpha", "zeta", "gamma")
     SCALAR = ("n_fri_layers", "final_len", "pow_witness", "pow_bits", "n_queries", "n_chips", "log_max")
     as_dict = SegmentProof.as_dict
+    from_dict = classmethod(SegmentProof.from_dict.__func__)
+
+
+class VerifyChip(C.Structure):
+    """pb_verify_chip_t"""
+    _fields_ = [("vk", C.c_void_p), ("log_n", C.c_size_t)]
+
+
+class VerifyParams(C.Structure):
+    """pb_verify_params_t"""
+    _fields_ = [("n_queries", C.c_uint32), ("pow_bits", C.c_uint32), ("rc_ext", C.c_void_p), ("rc_int", C.c_void_p), ("diag_m1", C.c_void_p)]
 
 
 STAGES = ("h2d", "lde", "merkle", "logup_gen", "logup_commit", "quotient", "qlde", "qmerkle", "open", "fri", "pow", "total")
@@ -209,6 +236,72 @@ class Air:
         if self.h:
             self.ctx.lib.pb_air_free(self.h)
             self.h = None
+
+
+class VerifyingKey:
+    """pb_vk_t: what the host verifier reads of an AIR, from the same (bytecode, spans, width, bus) as Context.air.  Needs no GPU."""
+
+    def __init__(self, bytecode, spans, width, bus=None):
+        self.lib = load_library()
+        bc = _u32(bytecode)
+        sp = (Span * max(1, len(spans)))(*[Span(o, l) for o, l in spans])
+        ints, isp, ibc = bus if bus and len(bus[0]) else ([], [], [])
+        ibc = _u32(ibc)
+        spn = (Span * max(1, len(isp)))(*[Span(o, l) for o, l in isp])
+        di = (DevInteraction * max(1, len(ints)))(*[DevInteraction(b, n, o) for b, n, o in ints])
+        h = C.c_void_p()
+        _chk(self.lib.pb_vk_create(bc.ctypes.data_as(C.c_void_p), C.c_size_t(bc.size), sp, C.c_size_t(len(spans)), C.c_uint32(width),
+                                   ibc.ctypes.data_as(C.c_void_p), C.c_size_t(ibc.size), spn, C.c_size_t(len(isp)), di, C.c_size_t(len(ints)),
+                                   C.byref(h)), "pb_vk_create")
+        self.h = h
+
+    def free(self):
+        if self.h:
+            self.lib.pb_vk_free(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.free()
+        except Exception:
+            pass
+
+
+def _verify_params(n_queries, pow_bits, poseidon2):
+    """-> (pb_verify_params_t, keep-alive); poseidon2 = (rc_ext [8][16], rc_int [13], diag_m1 [16]) canonical, or None for the default"""
+    prm = VerifyParams(n_queries, pow_bits, None, None, None)
+    keep = [_u32(a) for a in poseidon2] if poseidon2 is not None else []
+    if keep:
+        assert keep[0].size == 128 and keep[1].size == 13 and keep[2].size == 16
+        prm.rc_ext, prm.rc_int, prm.diag_m1 = [a.ctypes.data for a in keep]
+    return prm, keep
+
+
+def verify_chips(chips, proof, cumsums, ys, queries, n_queries=100, pow_bits=16, poseidon2=None):
+    """pb_verify_chips on the host: chips [(VerifyingKey, log_n)]; proof, cumulative sums, opened values and queries as
+    Context.prove_chips returns them; n_queries / pow_bits: the security parameters the proof must have.
+    -> (rc, reason): (0, 0) accepted, (PB_ERR_REJECTED, the failed check), or (PB_ERR_INVALID_ARG, 0)"""
+    lib = load_library()
+    arr = (VerifyChip * max(1, len(chips)))(*[VerifyChip(vk.h.value, int(ln)) for vk, ln in chips])
+    p = proof if isinstance(proof, ChipsProof) else ChipsProof.from_dict(proof)
+    prm, keep = _verify_params(n_queries, pow_bits, poseidon2)
+    cs, y, q = _u32(cumsums), _u32(ys), _u32(queries)
+    reason = C.c_int()
+    rc = lib.pb_verify_chips(arr, C.c_size_t(len(chips)), C.byref(prm), C.byref(p), cs.ctypes.data_as(C.c_void_p), y.ctypes.data_as(C.c_void_p),
+                             C.c_size_t(y.size), q.ctypes.data_as(C.c_void_p), C.c_size_t(q.size), C.byref(reason))
+    return rc, reason.value
+
+
+def verify_segment(vk, log_n, proof, ys, queries, n_queries=100, pow_bits=16, poseidon2=None):
+    """pb_verify_segment: a proof, opened values and queries as Context.prove_segment / query_segment return them -> (rc, reason)"""
+    lib = load_library()
+    p = proof if isinstance(proof, SegmentProof) else SegmentProof.from_dict(proof)
+    prm, keep = _verify_params(n_queries, pow_bits, poseidon2)
+    y, q = _u32(ys), _u32(queries)
+    reason = C.c_int()
+    rc = lib.pb_verify_segment(vk.h, C.c_size_t(log_n), C.byref(prm), C.byref(p), y.ctypes.data_as(C.c_void_p), C.c_size_t(y.size),
+                               q.ctypes.data_as(C.c_void_p), C.c_size_t(q.size), C.byref(reason))
+    return rc, reason.value
 
 
 class Context:

@@ -2,7 +2,8 @@
 // live in the .cuh files included below.  Host code here plays the role of the reference's Rust host side
 // (bytecode packing ~ emit_expr, /root/reference/openvm/src/powdr_extension/trace_generator/cuda/mod.rs:49-81;
 // launch wrappers ~ /root/reference/openvm/src/cuda_abi.rs:97-135,174-223; stage order ~ engine.prove behind
-// /root/reference/openvm-riscv/src/lib.rs:327-332).  No CPU fallback exists: every entry point needs a CUDA device.
+// /root/reference/openvm-riscv/src/lib.rs:327-332).  No CPU fallback exists: every proving entry point needs a CUDA device.  The
+// verifier (verify.inl) is host code and needs none.
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdlib.h>
@@ -53,6 +54,14 @@ inline bb::E4 h_e4_from_canon(const uint32_t v[4]) { bb::E4 r; for (int i = 0; i
 // the transcript's permutation runs on the host (transcript_host.cpp: AVX-512 with a scalar fallback)
 using pbhost::P2Host;
 inline void host_permute(uint32_t s[16], const P2Host& k) { pbhost::permute(s, k); }
+// the host permutation's constants from canonical ones (pb_ctx_set_poseidon2's arguments)
+inline P2Host host_p2(const uint32_t rc_ext[8][16], const uint32_t rc_int[13], const uint32_t diag_m1[16]) {
+    P2Host k;
+    for (int r = 0; r < 8; r++) for (int i = 0; i < 16; i++) k.rc_ext[r][i] = h_to_m(rc_ext[r][i]);
+    for (int r = 0; r < 13; r++) k.rc_int[r] = h_to_m(rc_int[r]);
+    for (int i = 0; i < 16; i++) k.diag[i] = h_to_m(diag_m1[i]);
+    return k;
+}
 
 // DuplexChallenger<BabyBear, Perm16, 16, 8> on Montgomery values (SURVEY.md App. C.6)
 struct Challenger {
@@ -521,10 +530,7 @@ int pb_ctx_destroy(pb_ctx_t* ctx) {
 // the transcript's host-side permutation with the default (Plonky3) instance, canonical words in and out; needs no device
 int pb_host_poseidon2_permute(uint32_t state[16], int reps, int force_scalar, int* used_avx512) {
     if (!state || reps < 0) return PB_ERR_INVALID_ARG;
-    P2Host k;
-    for (int r = 0; r < 8; r++) for (int i = 0; i < 16; i++) k.rc_ext[r][i] = h_to_m(PB_P2_RC_EXT[r][i]);
-    for (int r = 0; r < 13; r++) k.rc_int[r] = h_to_m(PB_P2_RC_INT[r]);
-    for (int i = 0; i < 16; i++) k.diag[i] = h_to_m(PB_P2_DIAG_M1[i]);
+    const P2Host k = host_p2(PB_P2_RC_EXT, PB_P2_RC_INT, PB_P2_DIAG_M1);
     uint32_t s[16];
     for (int i = 0; i < 16; i++) s[i] = h_to_m(state[i]);
     for (int i = 0; i < reps; i++) { if (force_scalar) pbhost::permute_scalar(s, k); else pbhost::permute(s, k); }
@@ -1067,6 +1073,7 @@ int pb_deep_quotient(pb_ctx_t* ctx, const uint32_t* const* d_mats, const size_t*
 
 #include "segment.inl"
 #include "chips.inl"
+#include "verify.inl"
 
 int pb_last_stage_ms(pb_ctx_t* ctx, float ms[PB_N_STAGES]) {
     if (!ctx || !ms) return PB_ERR_INVALID_ARG;
