@@ -352,6 +352,51 @@ int pb_verify_chips(const pb_verify_chip_t* chips, size_t n_chips, const pb_veri
 int pb_verify_segment(const pb_vk_t* vk, size_t log_n, const pb_verify_params_t* params, const pb_segment_proof_t* proof,
                       const uint32_t* h_ys, size_t ys_words, const uint32_t* h_queries, size_t queries_words, int* reason);
 
+/* ---- a proof as bytes: what a prover publishes and a verifier on another machine reads (host code, no device, thread-safe) ----------
+ * One format for both provers: a segment proof is written as the one-chip multi-chip proof, so the blob of pb_prove_segment on a trace
+ * is byte for byte the blob of pb_prove_chips on that one chip.  The blob is a sequence of little-endian u32 words, field words canonical
+ * as in the proof structs, in this order (K = n_chips, L = n_fri_layers, F = final_len):
+ *   header       PB_PROOF_MAGIC, PB_PROOF_VERSION, K, n_queries, pow_bits, log_max, L, F, 0 (reserved)
+ *                per chip: log_n, width, perm_width                                                               9 + 3K words
+ *   proof        main_root, perm_root, quotient_root (8 each), logup_alpha, logup_beta, alpha, zeta, gamma (4 each),
+ *                fri_roots [L][8], fri_betas [L][4], final_poly [F][4], pow_witness                    44 + 12L + 4F + 1 words
+ *   cumsums      [K][4]
+ *   opened       [n_opened][4]                 n_opened = sum width + 2 * sum perm_width + 8K (pb_chips_sizes)
+ *   queries      [n_queries][words_per_query]  the layout of pb_chips_sizes / pb_query_chips for these chips
+ * so the blob's length follows from the header alone.  The blob carries the chips' widths and heights because its receiver holds only
+ * the verifying keys.  A blob is MALFORMED (PB_ERR_REJECTED, reason 23) if its magic or version differs, its length is not exactly the
+ * one its header gives (no trailing bytes), K is 0 or above PB_PROOF_MAX_CHIPS, a log_n is outside 1..24, a perm_width is neither 0 nor
+ * 4 * (chunks + 1) (a multiple of 4, at least 8), L is above 32 or F above 8 (the proof struct's arrays), the length computation
+ * overflows, or the reserved word is not zero.  The decoder checks all of that before it reads past the header. */
+#define PB_PROOF_MAGIC 0x46504250u     /* the bytes "PBPF" */
+#define PB_PROOF_VERSION 1u
+#define PB_PROOF_MAX_CHIPS 4096u
+typedef struct { uint32_t log_n, width, perm_width; } pb_proof_chip_t;
+/* The blob of a proof of pb_prove_chips / pb_prove_chips_sharded with the cumulative sums, opened values and queries of pb_query_chips:
+ * chips[c] = (log_n, width, pb_air_perm_width) of chip c.  out = NULL: only *len (bytes) is set.  PB_ERR_INVALID_ARG: NULL pointers,
+ * n_chips other than proof->n_chips, a shape the format cannot hold (see MALFORMED), ys_words / queries_words other than pb_chips_sizes
+ * gives (n_opened * 4, proof->n_queries * words_per_query), or capacity < *len.  Words are written as given: the verifier checks them. */
+int pb_chips_proof_encode(const pb_chips_proof_t* proof, const pb_proof_chip_t* chips, size_t n_chips, const uint32_t* h_cumsums,
+                          const uint32_t* h_ys, size_t ys_words, const uint32_t* h_queries, size_t queries_words, void* out, size_t capacity,
+                          size_t* len);
+/* the same blob for a proof of pb_prove_segment / pb_prove_segment_sharded with pb_last_openings and pb_query_segment(_sharded) */
+int pb_segment_proof_encode(const pb_segment_proof_t* proof, size_t log_n, size_t width, const uint32_t* h_ys, size_t ys_words,
+                            const uint32_t* h_queries, size_t queries_words, void* out, size_t capacity, size_t* len);
+/* decoding in two calls: pb_proof_bytes_sizes gives the blob's chip count and the lengths in words of its opened values and queries (the
+ * cumulative sums are 4 * n_chips words); the decoder then fills the struct, the chips' shapes and the three arrays, whose lengths must
+ * be exactly those (else PB_ERR_INVALID_ARG).  Both return PB_ERR_REJECTED with *reason 23 for a malformed blob.  pb_segment_proof_decode
+ * gives a one-chip blob back as a segment proof (its cumulative_sum, perm_width, log_n and width from the blob); another chip count, or
+ * a log_max other than log_n + 1, which the segment struct cannot hold, is reason 20. */
+int pb_proof_bytes_sizes(const void* bytes, size_t len, size_t* n_chips, size_t* ys_words, size_t* queries_words, int* reason);
+int pb_chips_proof_decode(const void* bytes, size_t len, pb_chips_proof_t* proof, pb_proof_chip_t* chips, size_t n_chips, uint32_t* h_cumsums,
+                          uint32_t* h_ys, size_t ys_words, uint32_t* h_queries, size_t queries_words, int* reason);
+int pb_segment_proof_decode(const void* bytes, size_t len, pb_segment_proof_t* proof, size_t* log_n, size_t* width, uint32_t* h_ys, size_t ys_words,
+                            uint32_t* h_queries, size_t queries_words, int* reason);
+/* decodes the blob and runs the checks of pb_verify_chips on it, chip c's key being vks[c] and its height the blob's: 23 a malformed blob;
+ * 20 also: a chip count other than n_vks, or a width or perm_width other than the key's; then every check and reason of pb_verify_chips,
+ * so a blob and the struct it encodes get the same verdict.  PB_ERR_INVALID_ARG: NULL pointers, n_vks = 0, bad params. */
+int pb_verify_proof_bytes(const pb_vk_t* const* vks, size_t n_vks, const pb_verify_params_t* params, const void* bytes, size_t len, int* reason);
+
 int _apc_tracegen(uint32_t* d_output, size_t output_height, const OriginalAir* d_original_airs, const Subst* d_subs,
                   size_t n_subs, int num_apc_calls);
 int _apc_apply_derived_expr(uint32_t* d_output, size_t output_height, int num_apc_calls, const DerivedExprSpec* d_specs,

@@ -21,9 +21,15 @@ EXPORTS = [
     "pb_prove_chips_sharded", "pb_query_chips_sharded", "pb_ctx_set_memory_budget", "pb_last_row_blocks", "pb_footprint_bytes",
     "pb_launch_count", "pb_leaf_kernel_profile", "_apc_tracegen", "_apc_apply_derived_expr", "_apc_apply_bus",
     "pb_vk_create", "pb_vk_free", "pb_verify_chips", "pb_verify_segment",
+    "pb_chips_proof_encode", "pb_segment_proof_encode", "pb_proof_bytes_sizes", "pb_chips_proof_decode", "pb_segment_proof_decode",
+    "pb_verify_proof_bytes",
 ]
 PB_ERR_INVALID_ARG = -1
 PB_ERR_REJECTED = -8
+PB_PROOF_MAGIC = 0x46504250
+PB_PROOF_VERSION = 1
+PB_PROOF_MAX_CHIPS = 4096
+REASON_MALFORMED = 23
 
 
 class LibraryMissing(RuntimeError):
@@ -34,6 +40,14 @@ class PbError(RuntimeError):
     def __init__(self, code, where):
         super().__init__("%s failed with code %d (%s)" % (where, code, "cudaError_t" if code > 0 else "PB_ERR"))
         self.code = code
+
+
+class ProofRejected(PbError):
+    """PB_ERR_REJECTED from a decoder: .reason is 23 for malformed bytes, 20 for a blob of another shape"""
+
+    def __init__(self, reason, where):
+        super().__init__(PB_ERR_REJECTED, "%s (reason %d)" % (where, reason))
+        self.reason = reason
 
 
 class Span(C.Structure):
@@ -116,6 +130,11 @@ class VerifyChip(C.Structure):
 class VerifyParams(C.Structure):
     """pb_verify_params_t"""
     _fields_ = [("n_queries", C.c_uint32), ("pow_bits", C.c_uint32), ("rc_ext", C.c_void_p), ("rc_int", C.c_void_p), ("diag_m1", C.c_void_p)]
+
+
+class ProofChip(C.Structure):
+    """pb_proof_chip_t: a chip's shape as the proof's byte form carries it"""
+    _fields_ = [("log_n", C.c_uint32), ("width", C.c_uint32), ("perm_width", C.c_uint32)]
 
 
 STAGES = ("h2d", "lde", "merkle", "logup_gen", "logup_commit", "quotient", "qlde", "qmerkle", "open", "fri", "pow", "total")
@@ -301,6 +320,79 @@ def verify_segment(vk, log_n, proof, ys, queries, n_queries=100, pow_bits=16, po
     reason = C.c_int()
     rc = lib.pb_verify_segment(vk.h, C.c_size_t(log_n), C.byref(prm), C.byref(p), y.ctypes.data_as(C.c_void_p), C.c_size_t(y.size),
                                q.ctypes.data_as(C.c_void_p), C.c_size_t(q.size), C.byref(reason))
+    return rc, reason.value
+
+
+# ---- the proof's byte form (include/powdr_b200.h) ----
+def _encode(call, where):
+    """call(out, capacity, len_ptr) twice: the size, then the bytes"""
+    n = C.c_size_t()
+    _chk(call(None, C.c_size_t(0), C.byref(n)), where)
+    out = C.create_string_buffer(n.value)
+    _chk(call(out, C.c_size_t(n.value), C.byref(n)), where)
+    return out.raw[:n.value]
+
+
+def encode_chips_proof(proof, chips, cumsums, ys, queries):
+    """pb_chips_proof_encode: proof, cumulative sums, opened values and queries as Context.prove_chips returns them; chips
+    [(log_n, width, perm_width)] -> bytes"""
+    lib = load_library()
+    p = proof if isinstance(proof, ChipsProof) else ChipsProof.from_dict(proof)
+    arr = (ProofChip * max(1, len(chips)))(*[ProofChip(*[int(v) for v in c]) for c in chips])
+    cs, y, q = _u32(cumsums), _u32(ys), _u32(queries if queries is not None else np.empty(0))
+    return _encode(lambda out, cap, n: lib.pb_chips_proof_encode(
+        C.byref(p), arr, C.c_size_t(len(chips)), cs.ctypes.data_as(C.c_void_p), y.ctypes.data_as(C.c_void_p), C.c_size_t(y.size),
+        q.ctypes.data_as(C.c_void_p), C.c_size_t(q.size), out, cap, n), "pb_chips_proof_encode")
+
+
+def encode_segment_proof(proof, log_n, width, ys, queries):
+    """pb_segment_proof_encode: a proof, opened values and queries as Context.prove_segment / query_segment return them -> bytes"""
+    lib = load_library()
+    p = proof if isinstance(proof, SegmentProof) else SegmentProof.from_dict(proof)
+    y, q = _u32(ys), _u32(queries)
+    return _encode(lambda out, cap, n: lib.pb_segment_proof_encode(
+        C.byref(p), C.c_size_t(log_n), C.c_size_t(width), y.ctypes.data_as(C.c_void_p), C.c_size_t(y.size), q.ctypes.data_as(C.c_void_p),
+        C.c_size_t(q.size), out, cap, n), "pb_segment_proof_encode")
+
+
+def decode_proof(blob, segment=False):
+    """pb_proof_bytes_sizes + pb_chips_proof_decode -> (proof dict, chips [(log_n, width, perm_width)], cumulative sums (K, 4),
+    opened values (n_opened, 4), queries (n_queries, words_per_query)); segment=True: pb_segment_proof_decode -> (segment proof dict,
+    log_n, width, opened values, queries).  Raises ProofRejected for bytes the decoder refuses."""
+    lib = load_library()
+    b = bytes(blob)
+    k, nys, nq, reason = C.c_size_t(), C.c_size_t(), C.c_size_t(), C.c_int()
+    rc = lib.pb_proof_bytes_sizes(b, C.c_size_t(len(b)), C.byref(k), C.byref(nys), C.byref(nq), C.byref(reason))
+    if rc == PB_ERR_REJECTED:
+        raise ProofRejected(reason.value, "pb_proof_bytes_sizes")
+    _chk(rc, "pb_proof_bytes_sizes")
+    n_q = int.from_bytes(b[12:16], "little")          # header word 3, of a blob the call above has checked
+    ys = np.empty((nys.value // 4, 4), dtype=np.uint32)
+    q = np.empty((n_q, nq.value // n_q if n_q else 0), dtype=np.uint32)
+    yp, qp = ys.ctypes.data_as(C.c_void_p), q.ctypes.data_as(C.c_void_p)
+    if segment:
+        proof, log_n, width = SegmentProof(), C.c_size_t(), C.c_size_t()
+        rc = lib.pb_segment_proof_decode(b, C.c_size_t(len(b)), C.byref(proof), C.byref(log_n), C.byref(width), yp, nys, qp, nq, C.byref(reason))
+        out = (proof, int(log_n.value), int(width.value), ys, q)
+    else:
+        proof, chips, cs = ChipsProof(), (ProofChip * k.value)(), np.empty((k.value, 4), dtype=np.uint32)
+        rc = lib.pb_chips_proof_decode(b, C.c_size_t(len(b)), C.byref(proof), chips, k, cs.ctypes.data_as(C.c_void_p), yp, nys, qp, nq,
+                                       C.byref(reason))
+        out = (proof, [(c.log_n, c.width, c.perm_width) for c in chips], cs, ys, q)
+    if rc == PB_ERR_REJECTED:
+        raise ProofRejected(reason.value, "pb_segment_proof_decode" if segment else "pb_chips_proof_decode")
+    _chk(rc, "pb_segment_proof_decode" if segment else "pb_chips_proof_decode")
+    return (out[0].as_dict(),) + out[1:]
+
+
+def verify_proof_bytes(vks, blob, n_queries=100, pow_bits=16, poseidon2=None):
+    """pb_verify_proof_bytes: vks [VerifyingKey], one per chip of the blob in its order -> (rc, reason) as verify_chips"""
+    lib = load_library()
+    arr = (C.c_void_p * max(1, len(vks)))(*[vk.h.value for vk in vks])
+    prm, keep = _verify_params(n_queries, pow_bits, poseidon2)
+    b = bytes(blob)
+    reason = C.c_int()
+    rc = lib.pb_verify_proof_bytes(arr, C.c_size_t(len(vks)), C.byref(prm), b, C.c_size_t(len(b)), C.byref(reason))
     return rc, reason.value
 
 

@@ -3,7 +3,7 @@
 // (bytecode packing ~ emit_expr, /root/reference/openvm/src/powdr_extension/trace_generator/cuda/mod.rs:49-81;
 // launch wrappers ~ /root/reference/openvm/src/cuda_abi.rs:97-135,174-223; stage order ~ engine.prove behind
 // /root/reference/openvm-riscv/src/lib.rs:327-332).  No CPU fallback exists: every proving entry point needs a CUDA device.  The
-// verifier (verify.inl) is host code and needs none.
+// verifier (verify.inl) and the proof's byte form (proof_bytes.inl) are host code and need none.
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdlib.h>
@@ -1074,6 +1074,7 @@ int pb_deep_quotient(pb_ctx_t* ctx, const uint32_t* const* d_mats, const size_t*
 #include "segment.inl"
 #include "chips.inl"
 #include "verify.inl"
+#include "proof_bytes.inl"
 
 int pb_last_stage_ms(pb_ctx_t* ctx, float ms[PB_N_STAGES]) {
     if (!ctx || !ms) return PB_ERR_INVALID_ARG;
