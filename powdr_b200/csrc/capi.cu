@@ -158,8 +158,9 @@ struct pb_bus {
 
 // one chip of a proof (chips.inl): its matrices stay resident until the query phase.  pb_prove_segment uses slot 0.  The sharded provers
 // (shard_api.inl) hold their row blocks here; their `perm` is [my trace rows x the padded permutation columns | row sums | my permutation
-// columns, whole].  A chip proved in 2^lb row blocks (lb > 0, single GPU) keeps its main coefficients in `coef` and its permutation
-// coefficients in `perm`; `lde` and `perm_lde` hold one row block, recomputed by each phase that reads it (rowblock.inl).
+// columns, whole].  On one GPU a chip's LDEs are 2^lb row blocks (rowblock.inl), and `lde` and `perm_lde` hold one of them: a resident
+// chip (lb = 0) has one block, its whole LDE; a row-blocked chip (lb > 0) keeps its main coefficients in `coef` and its permutation
+// coefficients in `perm`, and each phase that reads a block recomputes it.
 struct McChip {
     size_t log_n = 0, width = 0, wp = 0, n_chunks = 0, e_main = 0, e_perm = 0, e_q = 0, lb = 0;
     const pb_air* air = nullptr;
@@ -168,7 +169,9 @@ struct McChip {
     bb::E4 cumsum = {{0u, 0u, 0u, 0u}};
 };
 
-struct Mat { const uint32_t* p; size_t width; size_t log_h; };      // a committed matrix, column-major [width][2^log_h]
+// a committed matrix, column-major [width][2^log_h]; w: the chip whose main (perm = false) or permutation LDE it is, when each of its row
+// blocks is to be recomputed into p before it is read (lde_block)
+struct Mat { const uint32_t* p; size_t width; size_t log_h; McChip* w = nullptr; bool perm = false; };
 
 namespace shard { struct Xfer; }        // one chip's slice of a batched exchange (shard_api.inl)
 
