@@ -401,20 +401,24 @@ size_t lde_column_batch(const pb_ctx* ctx, size_t N, size_t width) {
     return (width + (width + batch - 1) / batch - 1) / ((width + batch - 1) / batch);     // equal-sized batches (no runt batch)
 }
 
-// K1 + K2a: nb natural-order columns (stride N) -> coefficients in bit-reversed slots, scaled by 1/N, in coef (stride N)
+// K1: inverse high bits, nb natural-order columns (stride N) of src into coef (stride N)
 template <int LOG_N>
-void inverse_passes(pb_ctx* ctx, const TwiddleSet* tw, const uint32_t* src, unsigned nb, uint32_t* coef) {
+void k1_pass(pb_ctx* ctx, const TwiddleSet* tw, const uint32_t* src, unsigned nb, uint32_t* coef) {
     constexpr int LO = nttf::n_lo_of(LOG_N), HI = LOG_N - LO;
     constexpr size_t N = (size_t)1 << LOG_N;
-    if constexpr (HI > 0) {
-        const dim3 g1(1u << (LO - nttf::log_lc_of(HI)), nb);
-        nttf::strided_kernel<HI, LO, true><<<g1, nttf::THREADS, nttf::tile_bytes(HI), ctx->stream>>>(src, N, coef, N, 0, tw->d_inv);
-        LAUNCHED(ctx);
-        src = coef;
-    }
+    const dim3 g1(1u << (LO - nttf::log_lc_of(HI)), nb);
+    nttf::strided_kernel<HI, LO, true><<<g1, nttf::THREADS, nttf::tile_bytes(HI), ctx->stream>>>(src, N, 0u, coef, N, 0, tw->d_inv);
+    LAUNCHED(ctx);
+}
+
+// K2a: inverse low bits, src (stride N; may be coef) into coef (stride N), scaled by 1/N
+template <int LOG_N>
+void k2a_pass(pb_ctx* ctx, const TwiddleSet* tw, const uint32_t* src, unsigned nb, uint32_t* coef) {
+    constexpr int LO = nttf::n_lo_of(LOG_N), HI = LOG_N - LO;
+    constexpr size_t N = (size_t)1 << LOG_N;
     const size_t total_blocks = (size_t)nb << HI;
     // n_lo == 10: the TMA-staged kernel (ntt_tma.cuh) where its preconditions hold
-    if (!ntttma::launch_transposed(true, LOG_N, LO, ctx->stream, src, coef, 0, total_blocks, nb * N, nb * N, tw->d_inv, tw->ninv)) {
+    if (!ntttma::launch_inverse(LOG_N, LO, ctx->stream, src, coef, nb, tw->d_inv, tw->ninv)) {
         const dim3 g2((unsigned)((total_blocks + ((size_t)1 << nttf::log_lc_of(LO)) - 1) >> nttf::log_lc_of(LO)));
         nttf::transposed_kernel<LO, true><<<g2, nttf::THREADS, nttf::tile_bytes(LO), ctx->stream>>>(src, N, coef, LOG_N, 0, total_blocks,
                                                                                                     tw->d_inv, tw->ninv);
@@ -422,31 +426,75 @@ void inverse_passes(pb_ctx* ctx, const TwiddleSet* tw, const uint32_t* src, unsi
     LAUNCHED(ctx);
 }
 
-// K2b + K3: coefficients (bit-reversed slots, stride N) -> 2^log_blowup coset evaluations per column, bit-reversed rows,
-// out[col * out_stride + bitrev_b(c) * N + bitrev_n(k)];  scratch holds [nb][cosets][N]
+// K2b: forward low bits, coefficients (stride N) -> scratch [nb][cosets][N]
 template <int LOG_N>
-void forward_passes(pb_ctx* ctx, const TwiddleSet* tw, int log_blowup, const uint32_t* coef, unsigned nb, uint32_t* scratch, uint32_t* out,
-                    size_t out_stride) {
+void k2b_pass(pb_ctx* ctx, const TwiddleSet* tw, int log_blowup, const uint32_t* coef, unsigned nb, uint32_t* scratch) {
     constexpr int LO = nttf::n_lo_of(LOG_N), HI = LOG_N - LO;
     constexpr size_t N = (size_t)1 << LOG_N;
-    const unsigned cosets = 1u << log_blowup;
     const size_t total_blocks = (size_t)nb << HI;
-    if (!ntttma::launch_transposed(false, LOG_N, LO, ctx->stream, coef, scratch, log_blowup, total_blocks, nb * N, nb * N * cosets, tw->d_fwd,
-                                   make_uint2(0u, 0u))) {
-        const dim3 g2((unsigned)((total_blocks + ((size_t)1 << nttf::log_lc_of(LO)) - 1) >> nttf::log_lc_of(LO)), 1, cosets);
-        nttf::transposed_kernel<LO, false><<<g2, nttf::THREADS, nttf::tile_bytes(LO), ctx->stream>>>(coef, N, scratch, LOG_N, log_blowup,
-                                                                                                     total_blocks, tw->d_fwd, make_uint2(0u, 0u));
-    }
+    const dim3 g2((unsigned)((total_blocks + ((size_t)1 << nttf::log_lc_of(LO)) - 1) >> nttf::log_lc_of(LO)), 1, 1u << log_blowup);
+    nttf::transposed_kernel<LO, false><<<g2, nttf::THREADS, nttf::tile_bytes(LO), ctx->stream>>>(coef, N, scratch, LOG_N, log_blowup,
+                                                                                                 total_blocks, tw->d_fwd, make_uint2(0u, 0u));
     LAUNCHED(ctx);
+}
+
+// K3 (or, without high bits, the bit-reversed store): scratch [nb][cosets][N] -> out[col * out_stride + bitrev_b(c) * N + bitrev_n(k)];
+// the scratch rows are grouped by 2^lg (nttf::strided_kernel), 0 = natural order
+template <int LOG_N>
+void k3_pass(pb_ctx* ctx, const TwiddleSet* tw, int log_blowup, unsigned nb, const uint32_t* scratch, uint32_t lg, uint32_t* out, size_t out_stride) {
+    constexpr int LO = nttf::n_lo_of(LOG_N), HI = LOG_N - LO;
+    const unsigned cosets = 1u << log_blowup;
     if constexpr (HI > 0) {
         const dim3 g3(1u << (LO - nttf::log_lc_of(HI)), nb, cosets);
-        nttf::strided_kernel<HI, LO, false><<<g3, nttf::THREADS, nttf::tile_bytes(HI), ctx->stream>>>(scratch, 0, out, out_stride, log_blowup,
+        nttf::strided_kernel<HI, LO, false><<<g3, nttf::THREADS, nttf::tile_bytes(HI), ctx->stream>>>(scratch, 0, lg, out, out_stride, log_blowup,
                                                                                                       tw->d_fwd);
     } else {
         const size_t tot = ((size_t)nb * cosets) << LOG_N;
         ntt::bitrev_store_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, ctx->stream>>>(scratch, out, out_stride, LOG_N, log_blowup, nb);
     }
     LAUNCHED(ctx);
+}
+
+// K1 + K2a: nb natural-order columns (stride N) -> coefficients in bit-reversed slots, scaled by 1/N, in coef (stride N)
+template <int LOG_N>
+void inverse_passes(pb_ctx* ctx, const TwiddleSet* tw, const uint32_t* src, unsigned nb, uint32_t* coef) {
+    if constexpr (LOG_N > nttf::n_lo_of(LOG_N)) {
+        k1_pass<LOG_N>(ctx, tw, src, nb, coef);
+        src = coef;
+    }
+    k2a_pass<LOG_N>(ctx, tw, src, nb, coef);
+}
+
+// K2b + K3: coefficients (bit-reversed slots, stride N) -> 2^log_blowup coset evaluations per column, bit-reversed rows,
+// out[col * out_stride + bitrev_b(c) * N + bitrev_n(k)];  scratch holds [nb][cosets][N]
+template <int LOG_N>
+void forward_passes(pb_ctx* ctx, const TwiddleSet* tw, int log_blowup, const uint32_t* coef, unsigned nb, uint32_t* scratch, uint32_t* out,
+                    size_t out_stride) {
+    k2b_pass<LOG_N>(ctx, tw, log_blowup, coef, nb, scratch);
+    k3_pass<LOG_N>(ctx, tw, log_blowup, nb, scratch, 0u, out, out_stride);
+}
+
+// the whole LDE of nb natural-order columns (stride N) into out: inverse_passes into tmp, then forward_passes through scratch, except
+// that where the TMA kernels apply (n_lo = 10) K2a and K2b run as one pass and the coefficients never reach HBM
+template <int LOG_N>
+void lde_passes(pb_ctx* ctx, const TwiddleSet* tw, int log_blowup, const uint32_t* src, unsigned nb, uint32_t* tmp, uint32_t* scratch,
+                uint32_t* out, size_t out_stride) {
+    constexpr int LO = nttf::n_lo_of(LOG_N);
+    if constexpr (LOG_N > LO) {
+        k1_pass<LOG_N>(ctx, tw, src, nb, tmp);
+        uint32_t lg = 0;
+        if (ntttma::launch_low_bits(LOG_N, LO, ctx->stream, tmp, scratch, nb, log_blowup, tw->d_inv, tw->ninv, tw->d_fwd)) {
+            LAUNCHED(ctx);
+            lg = ntttma::LOG_ROW_GROUP;
+        } else {
+            k2a_pass<LOG_N>(ctx, tw, tmp, nb, tmp);
+            k2b_pass<LOG_N>(ctx, tw, log_blowup, tmp, nb, scratch);
+        }
+        k3_pass<LOG_N>(ctx, tw, log_blowup, nb, scratch, lg, out, out_stride);
+    } else {
+        inverse_passes<LOG_N>(ctx, tw, src, nb, tmp);
+        forward_passes<LOG_N>(ctx, tw, log_blowup, tmp, nb, scratch, out, out_stride);
+    }
 }
 
 // dynamic shared memory opt-in of the passes' kernels on the current device
@@ -465,11 +513,12 @@ int opt_in_passes() {
 struct NttPlan {
     void (*inverse)(pb_ctx*, const TwiddleSet*, const uint32_t*, unsigned, uint32_t*);
     void (*forward)(pb_ctx*, const TwiddleSet*, int, const uint32_t*, unsigned, uint32_t*, uint32_t*, size_t);
+    void (*lde)(pb_ctx*, const TwiddleSet*, int, const uint32_t*, unsigned, uint32_t*, uint32_t*, uint32_t*, size_t);
     int (*opt_in)();
 };
 template <size_t... I>
 constexpr std::array<NttPlan, sizeof...(I)> make_ntt_plans(std::index_sequence<I...>) {
-    return {{{inverse_passes<(int)I + 1>, forward_passes<(int)I + 1>, opt_in_passes<(int)I + 1>}...}};
+    return {{{inverse_passes<(int)I + 1>, forward_passes<(int)I + 1>, lde_passes<(int)I + 1>, opt_in_passes<(int)I + 1>}...}};
 }
 constexpr auto NTT_PLANS = make_ntt_plans(std::make_index_sequence<24>());     // NTT_PLANS[log_n - 1], 1 <= log_n <= 24
 
@@ -479,6 +528,10 @@ void ntt_inverse_cols(pb_ctx* ctx, int log_n, const TwiddleSet* tw, const uint32
 void ntt_forward_cols(pb_ctx* ctx, int log_n, const TwiddleSet* tw, int log_blowup, const uint32_t* coef, unsigned nb, uint32_t* scratch,
                       uint32_t* out, size_t out_stride) {
     NTT_PLANS[log_n - 1].forward(ctx, tw, log_blowup, coef, nb, scratch, out, out_stride);
+}
+void ntt_lde_cols(pb_ctx* ctx, int log_n, const TwiddleSet* tw, int log_blowup, const uint32_t* src, unsigned nb, uint32_t* tmp, uint32_t* scratch,
+                  uint32_t* out, size_t out_stride) {
+    NTT_PLANS[log_n - 1].lde(ctx, tw, log_blowup, src, nb, tmp, scratch, out, out_stride);
 }
 
 }  // namespace
@@ -506,8 +559,8 @@ int pb_ctx_create(pb_ctx_t** out, int device, void* cuda_stream) {
         for (int i = 0; i < pb_ctx::KPROF; i++) { CK(cudaEventCreate(&ctx->kp_a[i])); CK(cudaEventCreate(&ctx->kp_b[i])); }
         // the runtime applies a kernel's shared memory opt-in to the current device only: every context does its own
         for (const NttPlan& p : NTT_PLANS) RC(p.opt_in());
-        CK(cudaFuncSetAttribute(ntttma::transposed_tma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, ntttma::SMEM_BYTES));
-        CK(cudaFuncSetAttribute(ntttma::transposed_tma_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, ntttma::SMEM_BYTES));
+        CK(cudaFuncSetAttribute(ntttma::transposed_tma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ntttma::SMEM_BYTES));
+        CK(cudaFuncSetAttribute(ntttma::lde_low_bits_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ntttma::LOW_BITS_SMEM_BYTES));
         return upload_p2(ctx, PB_P2_RC_EXT, PB_P2_RC_INT, PB_P2_DIAG_M1);
     };
     const int rc = init();
@@ -603,8 +656,7 @@ int pb_lde_batch(pb_ctx_t* ctx, const uint32_t* d_trace, size_t log_n, size_t wi
     rc = ctx->tmp2.ensure(batch * N * cosets); if (rc) return rc;
     for (size_t c0 = 0; c0 < width; c0 += batch) {
         const unsigned nb = (unsigned)std::min(batch, width - c0);
-        ntt_inverse_cols(ctx, n, tw, d_trace + c0 * N, nb, ctx->tmp.p);
-        ntt_forward_cols(ctx, n, tw, (int)log_blowup, ctx->tmp.p, nb, ctx->tmp2.p, d_lde + c0 * N * cosets, N * cosets);
+        ntt_lde_cols(ctx, n, tw, (int)log_blowup, d_trace + c0 * N, nb, ctx->tmp.p, ctx->tmp2.p, d_lde + c0 * N * cosets, N * cosets);
     }
     CK(cudaGetLastError());
     return 0;

@@ -13,7 +13,8 @@
 //       K2b forward, bits [0,n_lo)   per coset, same geometry
 //       K3  forward, bits [n_lo,n)   per coset, strided tiles, then the bit-reversed store
 //     Each pass reads and writes its column batch through HBM (11 words per element at b = 1); the batch is sized to fill the
-//     SMs, not to keep the intermediates in the 50 MB L2 (smaller, L2-sized batches measured no faster, capi.cu).
+//     SMs, not to keep the intermediates in the 50 MB L2 (smaller, L2-sized batches measured no faster, capi.cu).  At n_lo = 10
+//     pb_lde_batch runs K2a and K2b as one pass that keeps the coefficients on chip (ntt_tma.cuh): 9 words per element.
 //   * inside a pass the butterfly network never crosses lanes: a thread owns 2^q (q<=5) rows of one lane in REGISTERS and
 //     runs q radix-2 stages on them (80 butterflies per 32 loads + 32 stores for q=5); shared memory is touched once per
 //     round, conflict-free (lane = bank, XOR swizzle for the two transposed accesses).

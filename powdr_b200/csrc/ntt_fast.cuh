@@ -80,10 +80,12 @@ __device__ __forceinline__ void stages(uint32_t (&x)[1 << Q], const uint2* __res
     }
 }
 
-// one register round over a [2^RB rows][2^LLC lanes] tile; UB = global bit index of row bit 0 (NLO strided, 0 transposed)
+// one register round over a [2^RB rows][2^LLC lanes] tile; UB = global bit index of row bit 0 (NLO strided, 0 transposed).
+// G_IN reads row t of the tile at gsrc + ((t >> lg) << (UB + lg)) + ((t mod 2^lg) << LLC): lg = 0 natural order, else the rows of
+// the tile's lanes come in contiguous groups of 2^lg (K3 after ntttma::lde_low_bits_kernel).
 template <int RB, int LLC, int Q, int B0, int UB, bool INV, int SWZ, bool LANE_K, bool G_IN, bool G_OUT>
 __device__ __forceinline__ void round_dev(uint32_t* __restrict__ sm, const uint2* __restrict__ tw, uint2 ninv,
-                                          const uint32_t* __restrict__ gsrc, uint32_t* __restrict__ gdst, uint32_t live) {
+                                          const uint32_t* __restrict__ gsrc, uint32_t lg, uint32_t* __restrict__ gdst, uint32_t live) {
     constexpr uint32_t LC = 1u << LLC;
     constexpr uint32_t TASKS = (1u << (RB - Q)) << LLC;
     constexpr int KS = 1 << (B0 + UB);
@@ -97,7 +99,7 @@ __device__ __forceinline__ void round_dev(uint32_t* __restrict__ sm, const uint2
 #pragma unroll
         for (int e = 0; e < (1 << Q); e++) {
             const uint32_t t = tbase + ((uint32_t)e << B0);
-            x[e] = G_IN ? __ldg(gsrc + ((size_t)t << UB) + j) : sm[sidx<RB, LLC, SWZ>(t, j)];
+            x[e] = G_IN ? __ldg(gsrc + ((size_t)(t >> lg) << (UB + lg)) + ((t & ((1u << lg) - 1)) << LLC) + j) : sm[sidx<RB, LLC, SWZ>(t, j)];
         }
         const uint32_t koff = (LANE_K ? j : 0u) + (tl << UB);
         stages<Q, INV, KS, INV && UB == 0 && B0 == 0>(x, tw, UB + B0, koff, ninv);
@@ -112,21 +114,24 @@ __device__ __forceinline__ void round_dev(uint32_t* __restrict__ sm, const uint2
 
 // all rounds of a pass, unrolled at compile time in processing order (inverse: high bits first; forward: low bits first)
 template <int RB, int LLC, int UB, bool INV, int SWZ, bool LANE_K, bool G_FIRST, bool G_LAST, int I = 0>
-__device__ __forceinline__ void pass_rounds(uint32_t* sm, const uint2* tw, uint2 ninv, const uint32_t* gsrc, uint32_t* gdst,
+__device__ __forceinline__ void pass_rounds(uint32_t* sm, const uint2* tw, uint2 ninv, const uint32_t* gsrc, uint32_t lg, uint32_t* gdst,
                                             uint32_t live) {
     constexpr int NR = n_rounds(RB);
     if constexpr (I < NR) {
         constexpr int R = INV ? NR - 1 - I : I;
         constexpr bool gi = G_FIRST && I == 0, go = G_LAST && I == NR - 1;
-        round_dev<RB, LLC, q_of(RB, R), b0_of(RB, R), UB, INV, SWZ, LANE_K, gi, go>(sm, tw, ninv, gsrc, gdst, live);
+        round_dev<RB, LLC, q_of(RB, R), b0_of(RB, R), UB, INV, SWZ, LANE_K, gi, go>(sm, tw, ninv, gsrc, lg, gdst, live);
         if constexpr (I + 1 < NR) __syncthreads();
-        pass_rounds<RB, LLC, UB, INV, SWZ, LANE_K, G_FIRST, G_LAST, I + 1>(sm, tw, ninv, gsrc, gdst, live);
+        pass_rounds<RB, LLC, UB, INV, SWZ, LANE_K, G_FIRST, G_LAST, I + 1>(sm, tw, ninv, gsrc, lg, gdst, live);
     }
 }
 
-// K1 (INV) / K3 (!INV): strided tile, rows <-> position bits [NLO, NLO+RB), lane j <-> position j0 + j
+// K1 (INV) / K3 (!INV): strided tile, rows <-> position bits [NLO, NLO+RB), lane j <-> position j0 + j.
+// K3's source rows come in groups of 2^lg (0 for natural order; K1 ignores lg and reads natural order): position k = j + (t << NLO) of a coset is at word
+// ((t >> lg) << (NLO + lg)) + ((j >> LLC) << (LLC + lg)) + ((t mod 2^lg) << LLC) + (j mod 2^LLC), so a tile reads 2^lg rows of its
+// lanes as one contiguous piece instead of 2^lg pieces of 2^LLC words
 template <int RB, int NLO, bool INV>
-__global__ void __launch_bounds__(THREADS) strided_kernel(const uint32_t* __restrict__ src, size_t src_col_stride,
+__global__ void __launch_bounds__(THREADS) strided_kernel(const uint32_t* __restrict__ src, size_t src_col_stride, uint32_t lg,
                                                           uint32_t* __restrict__ dst, size_t dst_col_stride, int log_blowup,
                                                           const uint2* __restrict__ tw_all) {
     extern __shared__ uint32_t sm[];
@@ -135,10 +140,10 @@ __global__ void __launch_bounds__(THREADS) strided_kernel(const uint32_t* __rest
     const uint32_t j0 = blockIdx.x << LLC;
     const int c = INV ? 0 : (int)blockIdx.z;
     const int cosets = INV ? 1 : (1 << log_blowup);
-    const uint32_t* s = (INV ? src + (size_t)blockIdx.y * src_col_stride : src + (((size_t)blockIdx.y * cosets + c) << n)) + j0;
+    const uint32_t* s = INV ? src + (size_t)blockIdx.y * src_col_stride + j0 : src + (((size_t)blockIdx.y * cosets + c) << n) + ((size_t)j0 << lg);
     const uint2* tw = tw_all + ((size_t)c << n) + j0;         // lane part of the twiddle index is the position j0 + j
     uint32_t* d1 = dst + (size_t)blockIdx.y * dst_col_stride + j0;
-    pass_rounds<RB, LLC, NLO, INV, INV ? SWZ_NONE : SWZ_TOP, true, true, INV>(sm, tw, make_uint2(0u, 0u), s, d1, 1u << LLC);
+    pass_rounds<RB, LLC, NLO, INV, INV ? SWZ_NONE : SWZ_TOP, true, true, INV>(sm, tw, make_uint2(0u, 0u), s, INV ? 0u : lg, d1, 1u << LLC);
     if (!INV) {
         __syncthreads();
         // natural evaluation index k = j0 + j + (t << NLO) of coset c lands at row  bitrev_b(c)*N + bitrev_n(k)
@@ -175,7 +180,7 @@ __global__ void __launch_bounds__(THREADS) transposed_kernel(const uint32_t* __r
         for (uint32_t t = lane; t < ROWS; t += 32) sm[sidx<RB, LLC, SWZ_LOW>(t, l)] = __ldg(p + t);
     }
     __syncthreads();
-    pass_rounds<RB, LLC, 0, INV, SWZ_LOW, false, false, false>(sm, tw, ninv, nullptr, nullptr, live);
+    pass_rounds<RB, LLC, 0, INV, SWZ_LOW, false, false, false>(sm, tw, ninv, nullptr, 0u, nullptr, live);
     __syncthreads();
     for (uint32_t l = warp; l < live; l += THREADS / 32) {
         const size_t b = b_first + l, col = b >> log_bpc, blk = b & (((size_t)1 << log_bpc) - 1);

@@ -32,9 +32,11 @@ def pass_work(name, n, blowup):
     n_lo = n if n <= 10 else (n + 1) // 2
     n_hi = n - n_lo
     N, B = 1 << n, 1 << blowup
-    inv = "true" in name.split("(")[0]
+    inv = "true" in name.split("(")[0] or "transposed_tma_kernel" in name      # the TMA kernel of that name is K2a only
     if "strided" in name:
         return ("K1 inverse high bits", 2, N // 2 * n_hi) if inv else ("K3 forward high bits", 2 * B, B * (N // 2) * n_hi)
+    if "lde_low_bits" in name:
+        return ("K2a+K2b low bits, fused", 1 + B, (1 + B) * (N // 2) * n_lo)
     if "transposed" in name:
         return ("K2a inverse low bits", 2, N // 2 * n_lo) if inv else ("K2b forward low bits", 1 + B, B * (N // 2) * n_lo)
     return ("other", 0, 0)
