@@ -207,7 +207,8 @@ int pb_query_chips(pb_ctx_t* ctx, uint32_t* h_queries, size_t queries_capacity_w
 /* the budget: by default the device's free memory at the call plus what the context's proof workspaces hold; `bytes` lowers it, 0
  * restores the default */
 int pb_ctx_set_memory_budget(pb_ctx_t* ctx, size_t bytes);
-/* log2 of the row blocks of the last pb_prove_segment / pb_prove_chips of the context: 0 for the resident path */
+/* log2 of the row blocks of the last pb_prove_segment / pb_prove_chips of the context, or of the sub-blocks of each rank block of the
+ * last sharded proof: 0 for the resident path */
 int pb_last_row_blocks(pb_ctx_t* ctx, uint32_t* log_blocks);
 /* the bytes the choice above counts for chips of these heights, widths and permutation widths (pb_air_perm_width) with device-resident
  * traces (not counted), every height with log_n >= log_blocks + 3 in 2^log_blocks row blocks (0: resident); needs no device */
@@ -249,7 +250,9 @@ int pb_prove_segment_sharded(pb_ctx_t* ctx, const pb_air_t* air, const uint32_t*
                              const pb_comm_t* comm, pb_segment_proof_t* proof);
 /* query phase of the last pb_prove_segment_sharded, collective over the same ranks: the same indices, layout (pb_query_words) and
  * words as pb_query_segment after pb_prove_segment on the gathered trace, on every rank.  A row and the bottom of its Merkle path come
- * from the rank that holds that row block, the top log2(world) levels from the subtree roots kept at commit time; one all-gather. */
+ * from the rank that holds that row block, the top log2(world) levels from the subtree roots kept at commit time; one all-gather.
+ * After a row-blocked proof (pb_last_row_blocks > 0) each sub-step that holds a queried row is exchanged again first: one all-to-all
+ * per blocked height and sub-step (two with a permutation trace), so comm->all_to_all is then required (else PB_ERR_INVALID_ARG). */
 int pb_query_segment_sharded(pb_ctx_t* ctx, const pb_comm_t* comm, uint32_t* h_out, size_t out_capacity_words);
 /* ALL chips of a segment under one transcript across the same ranks: the proof, cumulative sums, opened values and query words of
  * pb_prove_chips + pb_query_chips on the gathered traces, word for word, on every rank.  Every rank passes all chips in the same order;
@@ -262,9 +265,26 @@ int pb_query_segment_sharded(pb_ctx_t* ctx, const pb_comm_t* comm, uint32_t* h_o
 int pb_prove_chips_sharded(pb_ctx_t* ctx, const pb_chip_t* chips, size_t n_chips, const pb_comm_t* comm, pb_chips_proof_t* proof,
                            uint32_t* h_cumsums);
 /* collective over the same ranks, on every rank: the queries and opened values pb_query_chips returns after pb_prove_chips on the gathered
- * traces (layout: pb_chips_sizes); h_queries / h_ys may be NULL (no queries: no collective) */
+ * traces (layout: pb_chips_sizes); h_queries / h_ys may be NULL (no queries: no collective).  One all-gather; after a row-blocked proof
+ * also the all-to-alls of pb_query_segment_sharded's note, so comm->all_to_all is then required (else PB_ERR_INVALID_ARG). */
 int pb_query_chips_sharded(pb_ctx_t* ctx, const pb_comm_t* comm, uint32_t* h_queries, size_t queries_capacity_words, uint32_t* h_ys,
                            size_t ys_capacity_words);
+/* ---- device memory of the sharded provers (pb_prove_chips_sharded, pb_prove_segment_sharded) ----------------------------------
+ * Without a budget (pb_ctx_set_memory_budget 0, the default) every rank keeps its row block of every LDE resident.  With a nonzero
+ * budget, which EVERY RANK MUST BE GIVEN ALIKE (the ranks choose the same path from the chip shapes, the world and that number alone, with
+ * no collective and without reading free memory), a proof whose per-rank footprint does not fit is proved with each rank block in
+ * B = 2^log_blocks sub-blocks, G * B <= 16: the chips of the tallest heights keep the coefficients of the rank's columns and of its
+ * permutation columns and one sub-block of each LDE; each phase that reads an LDE runs sub-step k = 0..B-1 as one all-to-all that
+ * brings every rank its sub-block k, so the proof and every answer stay word for word those of the resident path.  The choice is the
+ * single-GPU rule: a height is blocked for all its chips or none and only if log_n >= log2(G) + log_blocks + 3; the smallest B first,
+ * then the fewest heights, tallest first.  If nothing fits, every rank returns cudaErrorMemoryAllocation (2) before any collective.
+ * A row-blocked proof first frees the workspaces an earlier proof of the context left.  pb_last_row_blocks reports log_blocks. */
+/* one rank's bytes of that choice for chips of these heights, widths and permutation widths on `world` ranks, every height with
+ * log_n >= log2(world) + log_blocks + 3 in 2^log_blocks sub-blocks (0: resident).  The caller's column share of the traces is not
+ * counted.  PB_ERR_INVALID_ARG: world not 2..16 and a power of two, world * 2^log_blocks > 16, a chip below 2^(log2(world) + 3) rows.
+ * Needs no device. */
+int pb_footprint_bytes_sharded(const size_t* log_n, const size_t* width, const size_t* perm_width, size_t n_chips, int world, uint32_t log_blocks,
+                               size_t* bytes);
 
 /* The Fiat-Shamir transcript (DuplexChallenger over Poseidon2, width 16, rate 8) runs on the HOST: absorbing the opened values is a
  * serial sponge (4363 dependent permutations for the keccak shape), so it uses an AVX-512 permutation with the whole state in one

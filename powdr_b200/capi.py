@@ -19,6 +19,7 @@ EXPORTS = [
     "pb_ctx_set_fri_params", "pb_air_set_interactions", "pb_air_perm_width", "pb_air_logup_compile_only", "pb_allgather_caps", "pb_bus_compile", "pb_bus_free", "pb_bus_apply",
     "pb_shard_columns", "pb_lde_shard", "pb_prove_segment_sharded", "pb_query_segment_sharded", "pb_prove_chips", "pb_chips_sizes", "pb_query_chips", "pb_host_poseidon2_permute",
     "pb_prove_chips_sharded", "pb_query_chips_sharded", "pb_ctx_set_memory_budget", "pb_last_row_blocks", "pb_footprint_bytes",
+    "pb_footprint_bytes_sharded",
     "pb_launch_count", "pb_leaf_kernel_profile", "_apc_tracegen", "_apc_apply_derived_expr", "_apc_apply_bus",
     "pb_vk_create", "pb_vk_free", "pb_verify_chips", "pb_verify_segment",
     "pb_chips_proof_encode", "pb_segment_proof_encode", "pb_proof_bytes_sizes", "pb_chips_proof_decode", "pb_segment_proof_decode",
@@ -150,6 +151,18 @@ def footprint_bytes(chips, log_blocks=0):
     ln, w, wp = [(C.c_size_t * k)(*[int(c[i]) for c in chips]) for i in range(3)]
     out = C.c_size_t()
     _chk(lib.pb_footprint_bytes(ln, w, wp, C.c_size_t(k), C.c_uint32(log_blocks), C.byref(out)), "pb_footprint_bytes")
+    return int(out.value)
+
+
+def footprint_bytes_sharded(chips, world, log_blocks=0):
+    """chips: [(log_n, width, perm_width)] -> one rank's device bytes pb_footprint_bytes_sharded counts for a proof of them on `world`
+    ranks with each rank block in 2^log_blocks sub-blocks (the caller's column share not included)"""
+    lib = load_library()
+    k = len(chips)
+    ln, w, wp = [(C.c_size_t * k)(*[int(c[i]) for c in chips]) for i in range(3)]
+    out = C.c_size_t()
+    _chk(lib.pb_footprint_bytes_sharded(ln, w, wp, C.c_size_t(k), C.c_int(world), C.c_uint32(log_blocks), C.byref(out)),
+         "pb_footprint_bytes_sharded")
     return int(out.value)
 
 
@@ -568,11 +581,12 @@ class Context:
         return ys, q
 
     def set_memory_budget(self, nbytes):
-        """device memory the single-GPU provers may use (0: free memory at the call + what the context holds)"""
+        """device memory the single-GPU provers may use (0: free memory at the call + what the context holds); nonzero also governs
+        the sharded provers, per rank, and must then be the same on every rank (0: they stay resident)"""
         _chk(self.lib.pb_ctx_set_memory_budget(self.h, C.c_size_t(int(nbytes))), "pb_ctx_set_memory_budget")
 
     def last_row_blocks(self):
-        """log2 of the row blocks of the last prove_segment / prove_chips (0: resident)"""
+        """log2 of the row blocks of the last prove_segment / prove_chips, or of the sub-blocks per rank of a sharded proof (0: resident)"""
         lb = C.c_uint32()
         _chk(self.lib.pb_last_row_blocks(self.h, C.byref(lb)), "pb_last_row_blocks")
         return int(lb.value)

@@ -200,10 +200,12 @@ struct pb_ctx {
     DevBuf<uint32_t> ws_mc_dig;           // digests of the shorter height groups until the tree reaches their level
     uint32_t n_queries = 100, pow_bits = 16;
     size_t mem_budget = 0;                // pb_ctx_set_memory_budget (0: free device memory + what the proof workspaces hold)
-    uint32_t last_lb = 0;                 // log2 of the row blocks of the last single-GPU proof (0: resident)
+    uint32_t last_lb = 0;                 // log2 of the row blocks of the last proof (0: resident); sharded: per rank block
     DevBuf<uint32_t> ws_fri_ch, ws_fri_log;  // device challenger state and the (root, beta) log of the FRI commit phase
     DevBuf<uint32_t> ws_sh_qall;             // every rank's share of the query openings
     DevBuf<shard::Xfer> ws_sh_tab;           // chip table of the batched exchanges
+    DevBuf<uint32_t> ws_sh_q, ws_sh_sub;     // row-blocked sharded quotient: the rank's [chip][4][Ms], one sub-block's q | S | phi
+    const pb_comm_t* sh_comm = nullptr;      // set while a sharded proof or query phase runs: row blocks are then exchanged sub-steps
     // The last proof, read by the query phase of the prover that made it (everything else stays resident on the device).
     enum class Prover { segment, chips, sharded, chips_sharded };
     struct {

@@ -169,18 +169,20 @@ def _run_ranks(world, body):
     return out
 
 
-def prove_chips_threads(world, chips, device=0, fri_params=(8, 4), want_queries=True, stats=None, comm_factory=None):
+def prove_chips_threads(world, chips, device=0, fri_params=(8, 4), want_queries=True, stats=None, comm_factory=None, budget=0):
     """Prove all chips of a segment under one transcript with `world` thread-ranks on one GPU (pb_prove_chips_sharded).  chips:
     [(trace canonical (W, N) uint32, bytecode, spans, bus or None)]; each rank compiles its own AIRs and passes its column block of
     every chip.  -> per rank the tuple of Context.prove_chips (proof dict, cumulative sums, opened values, queries or None).
     stats (optional list of `world` slots): per rank {"calls", "bytes", "launches", "stage_ms"} of the proof and query phase.
-    comm_factory(group, rank, ctx) (optional) makes the rank's Comm instead of a ThreadComm."""
+    comm_factory(group, rank, ctx) (optional) makes the rank's Comm instead of a ThreadComm.
+    budget: every rank's pb_ctx_set_memory_budget (0: resident); stats then also has "log_blocks", pb_last_row_blocks."""
     from .capi import Context
 
     def body(rank, group):
         ctx = Context(device)
         try:
             ctx.set_fri_params(*fri_params)
+            ctx.set_memory_budget(budget)
             airs, bufs, args = [], [], []
             for trace, bc, spans, bus in chips:
                 width, n = trace.shape
@@ -197,7 +199,7 @@ def prove_chips_threads(world, chips, device=0, fri_params=(8, 4), want_queries=
                 raise comm.error
             if stats is not None:
                 stats[rank] = {"calls": dict(getattr(comm, "calls", {})), "bytes": dict(getattr(comm, "bytes", {})),
-                               "launches": ctx.launch_count() - l0, "stage_ms": ctx.last_stage_ms()}
+                               "launches": ctx.launch_count() - l0, "stage_ms": ctx.last_stage_ms(), "log_blocks": ctx.last_row_blocks()}
             for a in airs:
                 a.free()
             return res
@@ -208,11 +210,12 @@ def prove_chips_threads(world, chips, device=0, fri_params=(8, 4), want_queries=
 
 
 def prove_segment_threads(world, trace, bytecode, spans, device=0, on_device=True, fri_params=(8, 4), bus=None, want_queries=False,
-                          stage_ms=None, stats=None):
+                          stage_ms=None, stats=None, budget=0):
     """Prove one segment with `world` thread-ranks on one GPU (parity harness).  trace: canonical (W, N) uint32.
     -> list of per-rank proof dicts (all equal); with want_queries, list of (proof dict, query openings) per rank.
     stage_ms (optional list of `world` slots): each rank's Context.last_stage_ms() after its proof.
-    stats (optional list of `world` slots): each rank's collective calls and bytes (ThreadComm.calls / .bytes) and kernel launches."""
+    stats (optional list of `world` slots): each rank's collective calls and bytes (ThreadComm.calls / .bytes), kernel launches and
+    "log_blocks" (pb_last_row_blocks).  budget: every rank's pb_ctx_set_memory_budget (0: resident)."""
     from .capi import Context
     width, n = trace.shape
     log_n = n.bit_length() - 1
@@ -221,6 +224,7 @@ def prove_segment_threads(world, trace, bytecode, spans, device=0, on_device=Tru
         ctx = Context(device)
         try:
             ctx.set_fri_params(*fri_params)
+            ctx.set_memory_budget(budget)
             air = ctx.air(bytecode, spans, width, bus)
             first, count = shard_columns(width, world, rank)
             comm = ThreadComm(group, rank, ctx)
@@ -238,7 +242,8 @@ def prove_segment_threads(world, trace, bytecode, spans, device=0, on_device=Tru
             if want_queries:
                 res = (res, ctx.query_segment_sharded(comm, log_n, width, air.perm_width))
             if stats is not None:
-                stats[rank] = {"calls": dict(comm.calls), "bytes": dict(comm.bytes), "launches": ctx.launch_count() - l0}
+                stats[rank] = {"calls": dict(comm.calls), "bytes": dict(comm.bytes), "launches": ctx.launch_count() - l0,
+                               "log_blocks": ctx.last_row_blocks()}
             if comm.error:
                 raise comm.error
             return res
