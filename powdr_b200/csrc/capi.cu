@@ -119,7 +119,6 @@ struct DevBuf {
         return 0;
     }
     void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
-    int fit(size_t n) { if (cap > n) release(); return ensure(n); }      // exactly n: a larger buffer of an earlier proof is freed
 };
 
 __global__ void to_monty_kernel(uint32_t* a, size_t n) {
@@ -205,7 +204,6 @@ struct pb_ctx {
     DevBuf<uint32_t> ws_sh_qall;             // every rank's share of the query openings
     DevBuf<shard::Xfer> ws_sh_tab;           // chip table of the batched exchanges
     DevBuf<uint32_t> ws_sh_q, ws_sh_sub;     // row-blocked sharded quotient: the rank's [chip][4][Ms], one sub-block's q | S | phi
-    const pb_comm_t* sh_comm = nullptr;      // set while a sharded proof or query phase runs: row blocks are then exchanged sub-steps
     // The last proof, read by the query phase of the prover that made it (everything else stays resident on the device).
     enum class Prover { segment, chips, sharded, chips_sharded };
     struct {
