@@ -188,11 +188,20 @@ typedef struct {
 } pb_chips_proof_t;                  /* all values canonical */
 /* h_cumsums: [n_chips][4] canonical (zero for chips without interactions) */
 int pb_prove_chips(pb_ctx_t* ctx, const pb_chip_t* chips, size_t n_chips, pb_chips_proof_t* proof, uint32_t* h_cumsums);
+/* pb_prove_chips with every chips[c].d_trace in HOST memory, in the same layout (Montgomery, column-major, width x 2^log_n): the same
+ * proof and cumulative sums, and pb_query_chips then returns the same opened values and query words, word for word.  The traces are
+ * copied to the device behind the work on them: their columns stream over PCIe in chunks, grouped by LDE height (tallest first), and
+ * the copy of a chunk overlaps the LDE and the leaf hashing of the one before (DESIGN.md §3b).  Pinned memory (pb_host_alloc) gives
+ * that overlap; pageable memory gives the same proof without it.  The library keeps its own device copy, counted in the footprint: the
+ * host buffers may be freed or overwritten as soon as the call returns.  Argument checks, error codes and the proof state as
+ * pb_prove_chips's (pb_query_chips answers for it).  pb_prove_segment without PB_TRACE_ON_DEVICE is the one-chip case. */
+int pb_prove_chips_host(pb_ctx_t* ctx, const pb_chip_t* chips, size_t n_chips, pb_chips_proof_t* proof, uint32_t* h_cumsums);
 /* n_opened Ext4 values; words per query of the layout
  *   [ r | main rows of all chips | main path (log_max x 8) | perm rows of the chips with interactions | perm path (tallest such chip) |
  *     quotient rows (8 per chip) | quotient path | per FRI layer i: pair (8), path ((log_max-1-i) x 8) ] */
 int pb_chips_sizes(const pb_chip_t* chips, size_t n_chips, size_t* n_opened, size_t* words_per_query);
-/* queries ([n_queries][words_per_query], may be NULL) and opened values ([n_opened][4], may be NULL) of the last pb_prove_chips */
+/* queries ([n_queries][words_per_query], may be NULL) and opened values ([n_opened][4], may be NULL) of the last pb_prove_chips or
+ * pb_prove_chips_host */
 int pb_query_chips(pb_ctx_t* ctx, uint32_t* h_queries, size_t queries_capacity_words, uint32_t* h_ys, size_t ys_capacity_words);
 
 /* ---- device memory of the single-GPU provers (pb_prove_segment, pb_prove_chips) ---------------------------------------------
@@ -202,8 +211,9 @@ int pb_query_chips(pb_ctx_t* ctx, uint32_t* h_queries, size_t queries_capacity_w
  * main and permutation commitments, the quotient, the reduced opening, the query phase) recomputes block by block.  The proof is the
  * same, word for word.  A height is blocked for all of its chips or none, and only if log_n >= log_blocks + 3.  The prover takes the
  * resident path when it fits, else the smallest B and, at that B, the fewest blocked heights (tallest first) that fit; if nothing fits
- * it returns cudaErrorMemoryAllocation (2) before launching anything.  A host-resident trace (pb_prove_segment without
- * PB_TRACE_ON_DEVICE) is copied whole to the device first and counts in the footprint. */
+ * it returns cudaErrorMemoryAllocation (2) before launching anything.  Host-resident traces (pb_prove_chips_host, pb_prove_segment
+ * without PB_TRACE_ON_DEVICE) count in the footprint as their device copies, plus on the resident path 16 x 2^(log_n + 1) words of
+ * sponge state per distinct height; on the row-blocked path they are copied whole to the device first. */
 /* the budget: by default the device's free memory at the call plus what the context's proof workspaces hold; `bytes` lowers it, 0
  * restores the default */
 int pb_ctx_set_memory_budget(pb_ctx_t* ctx, size_t bytes);

@@ -17,7 +17,7 @@ EXPORTS = [
     "pb_lde_batch", "pb_air_compile", "pb_air_free", "pb_air_is_jit", "pb_air_jit_compile_only", "pb_quotient", "pb_constraint_fold", "pb_merkle_commit",
     "pb_merkle_commit_rows8", "pb_poseidon2_permute", "pb_fri_fold", "pb_eval_at_point", "pb_deep_quotient", "pb_prove_segment", "pb_query_words", "pb_query_segment", "pb_last_openings", "pb_last_stage_ms",
     "pb_ctx_set_fri_params", "pb_air_set_interactions", "pb_air_perm_width", "pb_air_logup_compile_only", "pb_allgather_caps", "pb_bus_compile", "pb_bus_free", "pb_bus_apply",
-    "pb_shard_columns", "pb_lde_shard", "pb_prove_segment_sharded", "pb_query_segment_sharded", "pb_prove_chips", "pb_chips_sizes", "pb_query_chips", "pb_host_poseidon2_permute",
+    "pb_shard_columns", "pb_lde_shard", "pb_prove_segment_sharded", "pb_query_segment_sharded", "pb_prove_chips", "pb_prove_chips_host", "pb_chips_sizes", "pb_query_chips", "pb_host_poseidon2_permute",
     "pb_prove_chips_sharded", "pb_query_chips_sharded", "pb_ctx_set_memory_budget", "pb_last_row_blocks", "pb_footprint_bytes",
     "pb_footprint_bytes_sharded",
     "pb_launch_count", "pb_leaf_kernel_profile", "_apc_tracegen", "_apc_apply_derived_expr", "_apc_apply_bus",
@@ -540,14 +540,16 @@ class Context:
         _chk(self.lib.pb_last_openings(self.h, ys.ctypes.data_as(C.c_void_p), C.c_size_t(ys.size)), "pb_last_openings")
         return out, ys
 
-    def prove_chips(self, chips, want_queries=True):
-        """chips: [(Air, d_trace_ptr, log_n, width)], device-resident Montgomery traces.  All chips of a segment under one transcript
-        (pb_prove_chips).  -> (proof dict, cumulative sums (K, 4), opened values (n_opened, 4), queries (n_queries, words) or None)"""
+    def prove_chips(self, chips, want_queries=True, on_device=True):
+        """chips: [(Air, trace_ptr, log_n, width)], Montgomery traces, device-resident (pb_prove_chips) or, on_device=False, in host
+        memory (pb_prove_chips_host: the same proof, copied in behind the work; pinned memory overlaps the copy).  All chips of a segment
+        under one transcript.  -> (proof dict, cumulative sums (K, 4), opened values (n_opened, 4), queries (n_queries, words) or None)"""
         K = len(chips)
         arr = (Chip * K)(*[Chip(a.h.value, int(p), int(ln), int(w)) for a, p, ln, w in chips])
         proof = ChipsProof()
         cums = np.zeros((K, 4), dtype=np.uint32)
-        _chk(self.lib.pb_prove_chips(self.h, arr, C.c_size_t(K), C.byref(proof), cums.ctypes.data_as(C.c_void_p)), "pb_prove_chips")
+        name = "pb_prove_chips" if on_device else "pb_prove_chips_host"
+        _chk(getattr(self.lib, name)(self.h, arr, C.c_size_t(K), C.byref(proof), cums.ctypes.data_as(C.c_void_p)), name)
         n_open, wpq = C.c_size_t(), C.c_size_t()
         _chk(self.lib.pb_chips_sizes(arr, C.c_size_t(K), C.byref(n_open), C.byref(wpq)), "pb_chips_sizes")
         ys = np.empty((n_open.value, 4), dtype=np.uint32)
