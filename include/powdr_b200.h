@@ -296,6 +296,41 @@ int pb_query_chips_sharded(pb_ctx_t* ctx, const pb_comm_t* comm, uint32_t* h_que
 int pb_footprint_bytes_sharded(const size_t* log_n, const size_t* width, const size_t* perm_width, size_t n_chips, int world, uint32_t log_blocks,
                                size_t* bytes);
 
+/* ---- the sharded provers on the ranks of ONE process: a group of contexts -----------------------------------------------------
+ * One call proves all chips of a segment on `world` contexts (one per GPU, or several on one device), the way the reference proves a
+ * segment in one process (engine.prove on one host thread per VM instance).  The library owns the rank threads: each call starts one
+ * per rank, which runs pb_prove_chips_sharded (pb_query_chips_sharded) on its context with the group's collectives.  Those are
+ * stream-ordered device-to-device copies (cudaMemcpyPeerAsync, over NVLink between GPUs with peer access) behind the kernels that
+ * produce them: no communication library, no host staging, no callbacks to write.
+ * pb_group_create: world = 2, 4, 8 or 16 (else PB_ERR_UNSUPPORTED, checked before any context is read) distinct contexts (else
+ * PB_ERR_INVALID_ARG), rank r = ctxs[r]; contexts may share a device.  It enables peer access between every pair of their distinct
+ * devices that supports it.  The contexts stay the caller's: destroy the group first.  One call at a time per group, and no other use
+ * of its contexts while a call runs. */
+typedef struct pb_group pb_group_t;
+int pb_group_create(pb_ctx_t* const* ctxs, int world, pb_group_t** out);
+int pb_group_destroy(pb_group_t* group);
+/* chips[r]: rank r's n_chips entries, each with an AIR compiled on ctxs[r] and d_trace = rank r's column block
+ * pb_shard_columns(width, world, r) on ctxs[r]'s device (NULL when empty).  proof and h_cumsums are pb_prove_chips' output on the
+ * gathered traces.
+ *   Inputs: pb_prove_chips_sharded's contract, per rank.  Where the column blocks come from stays with the caller (each rank's
+ *     tracegen, or its own copies); they must stay valid until the last pb_query_chips_group.
+ *   Checked before any rank starts (no kernel, no collective) -> PB_ERR_INVALID_ARG: NULL arguments; every rank has the same
+ *     (log_n, width) and AIR permutation width per chip; every context has the same memory budget, n_queries and pow_bits.  Per-rank
+ *     arguments (a NULL d_trace where the rank holds columns, a NULL AIR) are each rank's own check, as in pb_prove_chips_sharded.
+ *   Output: from rank 0; every rank's proof struct and cumulative sums are compared with rank 0's, a difference is PB_ERR_INTERNAL.
+ *   Errors: the first error in rank order that is not PB_ERR_COMM, PB_ERR_COMM only if nothing else failed.  A rank that fails aborts
+ *     the call: every other rank leaves its pending or next collective with PB_ERR_COMM, so no rank is left waiting.  On return every
+ *     context's stream is idle and the group can be used again.
+ *   Results on each context: its rank's proof state, exactly as after pb_prove_chips_sharded (pb_last_row_blocks, pb_last_stage_ms
+ *     per context).  Any other prover run on one of the contexts invalidates the group's proof. */
+int pb_prove_chips_group(pb_group_t* group, const pb_chip_t* const* chips, size_t n_chips, pb_chips_proof_t* proof,
+                         uint32_t* h_cumsums);
+/* pb_query_chips' queries and opened values for the group's last proof (layout: pb_chips_sizes; h_queries / h_ys may be NULL), every
+ * rank's compared with rank 0's (PB_ERR_INTERNAL if they differ).  PB_ERR_INVALID_ARG without a proof of this group, or after another
+ * prover ran on one of its contexts. */
+int pb_query_chips_group(pb_group_t* group, uint32_t* h_queries, size_t queries_capacity_words, uint32_t* h_ys,
+                         size_t ys_capacity_words);
+
 /* The Fiat-Shamir transcript (DuplexChallenger over Poseidon2, width 16, rate 8) runs on the HOST: absorbing the opened values is a
  * serial sponge (4363 dependent permutations for the keccak shape), so it uses an AVX-512 permutation with the whole state in one
  * register when the CPU has it (scalar otherwise; PB_HOST_P2_SCALAR=1 forces scalar).  This entry applies that permutation `reps`

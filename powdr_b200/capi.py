@@ -24,8 +24,12 @@ EXPORTS = [
     "pb_vk_create", "pb_vk_free", "pb_verify_chips", "pb_verify_segment",
     "pb_chips_proof_encode", "pb_segment_proof_encode", "pb_proof_bytes_sizes", "pb_chips_proof_decode", "pb_segment_proof_decode",
     "pb_verify_proof_bytes",
+    "pb_group_create", "pb_group_destroy", "pb_prove_chips_group", "pb_query_chips_group",
 ]
 PB_ERR_INVALID_ARG = -1
+PB_ERR_UNSUPPORTED = -2
+PB_ERR_COMM = -6
+PB_ERR_INTERNAL = -7
 PB_ERR_REJECTED = -8
 PB_PROOF_MAGIC = 0x46504250
 PB_PROOF_VERSION = 1
@@ -652,3 +656,55 @@ class Context:
                                      C.c_void_p(d_ints_ptr), C.c_size_t(n_ints), C.c_void_p(d_spans_ptr), C.c_size_t(n_spans),
                                      C.c_uint32(var_bus), C.c_void_p(d_var), C.c_size_t(var_bins), C.c_uint32(t2_bus), C.c_void_p(d_t2),
                                      C.c_uint32(sz0), C.c_uint32(sz1), C.c_uint32(bw_bus), C.c_void_p(d_bw)), "_apc_apply_bus")
+
+
+class Group:
+    """pb_group_t: contexts that prove as the ranks of one process (pb_prove_chips_group).  The library runs one thread per rank and
+    exchanges device to device; rank r = ctxs[r].  The contexts stay the caller's: close the group before them."""
+
+    def __init__(self, ctxs):
+        self.lib = load_library()
+        self.ctxs = list(ctxs)
+        self.world = len(self.ctxs)
+        arr = (C.c_void_p * max(1, self.world))(*[c.h.value for c in self.ctxs])
+        h = C.c_void_p()
+        _chk(self.lib.pb_group_create(arr, C.c_int(self.world), C.byref(h)), "pb_group_create")
+        self.h = h
+        self._chips = None
+
+    def close(self):
+        if self.h:
+            self.lib.pb_group_destroy(self.h)
+            self.h = None
+
+    def prove_chips(self, chips, want_queries=True):
+        """chips[r]: rank r's [(Air, d_trace_ptr, log_n, width)] as Context.prove_chips_sharded takes them (d_trace_ptr: rank r's column
+        block on its context's device, 0 when empty).  -> the tuple of Context.prove_chips.  Ranks with different numbers of chips are
+        refused here with PB_ERR_INVALID_ARG: the C call takes one n_chips for all of them."""
+        if len(chips) != self.world:
+            raise ValueError("one list of chips per rank: %d ranks, %d lists" % (self.world, len(chips)))
+        K = len(chips[0])
+        if any(len(c) != K for c in chips):
+            raise PbError(PB_ERR_INVALID_ARG, "pb_prove_chips_group (n_chips differs between ranks)")
+        arrs = [(Chip * max(1, K))(*[Chip(a.h.value if a else None, int(p or 0), int(ln), int(w)) for a, p, ln, w in c]) for c in chips]
+        ptrs = (C.c_void_p * self.world)(*[C.addressof(a) for a in arrs])
+        proof = ChipsProof()
+        cums = np.zeros((K, 4), dtype=np.uint32)
+        _chk(self.lib.pb_prove_chips_group(self.h, ptrs, C.c_size_t(K), C.byref(proof), cums.ctypes.data_as(C.c_void_p)), "pb_prove_chips_group")
+        self._chips = (arrs[0], K)
+        ys, q = self.query_chips(want_queries)
+        return proof.as_dict(), cums, ys, q
+
+    def query_chips(self, want_queries=True):
+        """opened values and query openings of the group's last proof (pb_query_chips_group); its AIRs and traces must still be alive"""
+        if self._chips is None:
+            raise PbError(PB_ERR_INVALID_ARG, "pb_query_chips_group (no proof of this group)")
+        arr, K = self._chips
+        n_open, wpq = C.c_size_t(), C.c_size_t()
+        _chk(self.lib.pb_chips_sizes(arr, C.c_size_t(K), C.byref(n_open), C.byref(wpq)), "pb_chips_sizes")
+        nq = self.ctxs[0].n_queries
+        ys = np.empty((n_open.value, 4), dtype=np.uint32)
+        q = np.empty((nq, wpq.value), dtype=np.uint32) if want_queries and nq else None
+        _chk(self.lib.pb_query_chips_group(self.h, q.ctypes.data_as(C.c_void_p) if q is not None else None, C.c_size_t(q.size if q is not None else 0),
+                                           ys.ctypes.data_as(C.c_void_p), C.c_size_t(ys.size)), "pb_query_chips_group")
+        return ys, q

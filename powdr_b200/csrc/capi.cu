@@ -10,7 +10,10 @@
 #include <string.h>
 #include <algorithm>
 #include <array>
+#include <condition_variable>
 #include <memory>
+#include <mutex>
+#include <thread>
 #include <unordered_map>
 #include <utility>
 #include <vector>
@@ -200,6 +203,7 @@ struct pb_ctx {
     uint32_t n_queries = 100, pow_bits = 16;
     size_t mem_budget = 0;                // pb_ctx_set_memory_budget (0: free device memory + what the proof workspaces hold)
     uint32_t last_lb = 0;                 // log2 of the row blocks of the last proof (0: resident); sharded: per rank block
+    uint64_t proof_serial = 0;            // proofs begun on this context (invalidate_proofs): a group's query phase checks it is still its proof
     DevBuf<uint32_t> ws_fri_ch, ws_fri_log;  // device challenger state and the (root, beta) log of the FRI commit phase
     DevBuf<uint32_t> ws_sh_qall;             // every rank's share of the query openings
     DevBuf<shard::Xfer> ws_sh_tab;           // chip table of the batched exchanges
@@ -1238,5 +1242,6 @@ int pb_bus_apply(pb_ctx_t* ctx, const pb_bus_t* b, const uint32_t* d_trace, size
 
 #include "shard_api.inl"
 #include "rowblock.inl"
+#include "group.inl"
 
 }  // extern "C"

@@ -4,6 +4,9 @@ pointers and links no communication library itself.
   TorchComm   -- one process per GPU, torch.distributed (NCCL over NVLink/NVSwitch); what bench.py uses for --gpus N > 1
   ThreadComm  -- G threads of one process on ONE GPU, a barrier plus host staging; the single-GPU parity harness
                  (tests/test_gpu_sharded.py): same library code path as NCCL, no second GPU needed
+
+prove_chips_group runs the same provers without a pb_comm_t of ours: the library's group (pb_prove_chips_group) owns the rank threads
+and exchanges device to device.
 """
 import ctypes as C
 import threading
@@ -251,3 +254,47 @@ def prove_segment_threads(world, trace, bytecode, spans, device=0, on_device=Tru
             ctx.close()
 
     return _run_ranks(world, body)
+
+
+def prove_chips_group(world, chips, devices=None, fri_params=(8, 4), want_queries=True, stats=None, budget=0):
+    """prove_chips_threads through the library's group (pb_prove_chips_group): `world` contexts, rank r on devices[r] (default: all on
+    device 0), each with its own AIRs and its column block of every chip; one call proves on all of them, the library running the rank
+    threads and the device-to-device exchanges.  -> the list prove_chips_threads returns, one entry per rank: the group's answer, which the
+    library has checked equal on every rank.  stats (optional list of `world` slots): per rank {"launches", "stage_ms", "log_blocks"}.
+    budget: every rank's pb_ctx_set_memory_budget (0: resident)."""
+    from .capi import Context, Group
+    devices = list(devices) if devices is not None else [0] * world
+    ctxs, airs, bufs, args, group = [], [], [], [], None
+    try:
+        for rank in range(world):
+            ctx = Context(devices[rank])        # makes its device current: the AIRs and the column blocks below go there
+            ctxs.append(ctx)
+            ctx.set_fri_params(*fri_params)
+            ctx.set_memory_budget(budget)
+            mine = []
+            for trace, bc, spans, bus in chips:
+                width, n = trace.shape
+                air = ctx.air(bc, spans, width, bus)
+                first, count = shard_columns(width, world, rank)
+                buf = ctx.to_device(trace[first:first + count]) if count else None
+                airs.append(air)
+                bufs.append(buf)
+                mine.append((air, buf.ptr if buf else 0, n.bit_length() - 1, width))
+            args.append(mine)
+        group = Group(ctxs)
+        l0 = [c.launch_count() for c in ctxs]
+        res = group.prove_chips(args, want_queries=want_queries)
+        if stats is not None:
+            for r, c in enumerate(ctxs):
+                stats[r] = {"launches": c.launch_count() - l0[r], "stage_ms": c.last_stage_ms(), "log_blocks": c.last_row_blocks()}
+        return [res] * world
+    finally:
+        if group is not None:
+            group.close()
+        for a in airs:
+            a.free()
+        for b in bufs:
+            if b is not None:
+                b.free()
+        for c in ctxs:
+            c.close()
