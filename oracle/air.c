@@ -99,7 +99,8 @@ void orc_apc_apply_bus(const uint32_t* out, int num_apc_calls, const uint32_t* b
                        const orc_span_t* sp, uint32_t var_range_bus_id, uint32_t* var_hist, size_t var_num_bins,
                        uint32_t tuple2_bus_id, uint32_t* tuple2_hist, uint32_t sz0, uint32_t sz1,
                        uint32_t bitwise_bus_id, uint32_t* bitwise_hist) {
-    (void)sz0;
+    /* an interaction whose arguments are outside its table is counted nowhere (periphery.rs:179-236 refuses it); each component
+     * is bounded on its own, so an out-of-table argument never aliases into another entry's bin */
     for (int r = 0; r < num_apc_calls; r++)
         for (size_t i = 0; i < n_ints; i++) {
             orc_interaction_t it = ints[i];
@@ -108,19 +109,16 @@ void orc_apc_apply_bus(const uint32_t* out, int num_apc_calls, const uint32_t* b
             if (m == 0) continue;
             if (it.bus_id == var_range_bus_id) {
                 uint32_t value = ARG(1), max_bits = ARG(2);
-                uint32_t idx = (1u << max_bits) + value - 1u;
-                assert(idx < var_num_bins);
-                var_hist[idx] += m;
+                /* bin (1 << max_bits) + value - 1; all 2^max_bits bins of max_bits must fit in the table */
+                if (max_bits < 32 && (2ull << max_bits) - 1 <= var_num_bins && value < (1ull << max_bits))
+                    var_hist[(1u << max_bits) + value - 1u] += m;
             } else if (it.bus_id == tuple2_bus_id) {
                 uint32_t v0 = ARG(1), v1 = ARG(2);
-                tuple2_hist[v0 * sz1 + v1] += m;
+                if (v0 < sz0 && v1 < sz1) tuple2_hist[(size_t)v0 * sz1 + v1] += m;
             } else if (it.bus_id == bitwise_bus_id) {
                 uint32_t x = ARG(1), y = ARG(2), sel = ARG(4);
                 /* BitwiseOperationLookup<8> count layout [range 2^16 | xor 2^16] (dependency header, not in tree) */
-                uint32_t idx = (x << 8) | y;
-                if (sel == 0) bitwise_hist[idx] += m;
-                else if (sel == 1) bitwise_hist[65536u + idx] += m;
-                else assert(0 && "Invalid selector");
+                if (x < 256 && y < 256 && sel <= 1) bitwise_hist[sel * 65536u + ((x << 8) | y)] += m;
             }
 #undef ARG
         }

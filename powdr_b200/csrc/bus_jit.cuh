@@ -6,7 +6,9 @@
 //   variable range checker  [value, max_bits]            -> bin (1 << max_bits) + value - 1
 //   tuple range checker     [v0, v1]                     -> bin v0 * sz1 + v1
 //   bitwise lookup          [x, y, x^y, selector]        -> bin (x << 8 | y) (+ 2^16 when selector = 1)   (count layout [range | xor])
-// other buses (execution bridge, memory, pc lookup) are skipped; multiplicities are added with one warp-aggregated atomic per bin.
+// arguments outside their table (max_bits beyond it, value >= 2^max_bits, x or y >= 256, selector > 1, v0 >= sz0, v1 >= sz1) are counted
+// nowhere, as in _apc_apply_bus; other buses (execution bridge, memory, pc lookup) are skipped; multiplicities are added with one
+// warp-aggregated atomic per bin.
 #pragma once
 #include "logup_jit.cuh"
 
@@ -27,6 +29,11 @@ __device__ __forceinline__ void hist_add(u32* hist, u32 idx, u32 mult) {
     u32 total = 0;
     for (unsigned rem = peers; rem;) { int l = __ffs(rem) - 1; rem &= rem - 1; total += __shfl_sync(peers, mult, l); }
     if ((int)(threadIdx.x & 31) == leader) atomicAdd(hist + idx, total);
+}
+// bin of (value, max_bits), or ~0u (never < var_bins) when the pair is outside a table of var_bins bins: max_bits whose 2^max_bits
+// bins do not all fit, or value >= 2^max_bits.  A function, so that a literal max_bits of 32 or more is not a constant shift.
+__device__ __forceinline__ u32 var_bin(u32 value, u32 max_bits, u32 var_bins) {
+    return (max_bits < 32u && (2ull << max_bits) - 1ull <= var_bins && value < (1ull << max_bits)) ? (1u << max_bits) + value - 1u : ~0u;
 }
 )";
 
@@ -54,15 +61,16 @@ inline std::string generate(const std::vector<uint32_t>& code, const std::vector
             const std::string m = val(0);
             if (it.bus_id == var_bus && it.num_args >= 2) {
                 const std::string a = val(1), b = val(2);
-                snprintf(buf, sizeof buf, " { const u32 m = %s; if (m) { const u32 idx = (1u << (%s & 31u)) + %s - 1u; if (idx < var_bins) hist_add(var_hist, idx, m); } }\n", m.c_str(),
-                         b.c_str(), a.c_str());
+                snprintf(buf, sizeof buf, " { const u32 m = %s; if (m) { const u32 idx = var_bin(%s, %s, var_bins); if (idx < var_bins) hist_add(var_hist, idx, m); } }\n", m.c_str(),
+                         a.c_str(), b.c_str());
             } else if (it.bus_id == t2_bus && it.num_args >= 2) {
                 const std::string a = val(1), b = val(2);
-                snprintf(buf, sizeof buf, " { const u32 m = %s; if (m) { const u32 idx = %s * sz1 + %s; if (idx < sz0 * sz1) hist_add(t2_hist, idx, m); } }\n", m.c_str(), a.c_str(), b.c_str());
+                snprintf(buf, sizeof buf, " { const u32 m = %s; if (m) { const u32 t0 = %s, t1 = %s; if (t0 < sz0 && t1 < sz1) hist_add(t2_hist, t0 * sz1 + t1, m); } }\n", m.c_str(),
+                         a.c_str(), b.c_str());
             } else if (it.bus_id == bw_bus && it.num_args >= 4) {
                 const std::string x = val(1), y = val(2), sel = val(4);
-                snprintf(buf, sizeof buf, " { const u32 m = %s; if (m) { const u32 sel = %s; const u32 idx = ((%s << 8) | %s) + (sel == 1u ? 65536u : 0u); if (sel <= 1u && idx < 131072u) hist_add(bw_hist, idx, m); } }\n",
-                         m.c_str(), sel.c_str(), x.c_str(), y.c_str());
+                snprintf(buf, sizeof buf, " { const u32 m = %s; if (m) { const u32 x = %s, y = %s, sel = %s; if (x < 256u && y < 256u && sel <= 1u) hist_add(bw_hist, ((x << 8) | y) + sel * 65536u, m); } }\n",
+                         m.c_str(), x.c_str(), y.c_str(), sel.c_str());
             } else continue;
             body += buf;
         }

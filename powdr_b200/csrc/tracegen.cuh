@@ -111,18 +111,21 @@ __global__ void __launch_bounds__(128) apc_apply_bus_kernel(const uint32_t* __re
 #define PB_ARG(k) bb::from_monty(eval_expr(bc + spans[it.args_index_off + (k)].off, spans[it.args_index_off + (k)].len, trace, (size_t)r))
         const uint32_t m = PB_ARG(0);
         if (m == 0u) continue;
+        // arguments outside their table are counted nowhere (cpu/periphery.rs:179-236 refuses them): every component is bounded on
+        // its own, so no out-of-table argument can alias into another entry's bin
         if (it.bus_id == var_range_bus_id) {
             const uint32_t value = PB_ARG(1), max_bits = PB_ARG(2);
-            const uint32_t idx = (1u << max_bits) + value - 1u;     // VariableRangeChecker::add_count indexing (apc_apply_bus.cu:74)
-            if (idx < var_num_bins) hist_add(var_hist, idx, m);
+            // VariableRangeChecker::add_count indexing (apc_apply_bus.cu:74): bin (1 << max_bits) + value - 1; the 2^max_bits bins
+            // of max_bits must all fit in the table
+            if (max_bits < 32u && (2ull << max_bits) - 1ull <= var_num_bins && value < (1ull << max_bits))
+                hist_add(var_hist, (1u << max_bits) + value - 1u, m);
         } else if (it.bus_id == tuple2_bus_id) {
             const uint32_t v0 = PB_ARG(1), v1 = PB_ARG(2);
-            const uint32_t idx = v0 * sz1 + v1;                     // apc_apply_bus.cu:89
-            if (idx < sz0 * sz1) hist_add(tuple2_hist, idx, m);
+            if (v0 < sz0 && v1 < sz1) hist_add(tuple2_hist, v0 * sz1 + v1, m);     // apc_apply_bus.cu:89
         } else {
             const uint32_t x = PB_ARG(1), y = PB_ARG(2), sel = PB_ARG(4);
-            const uint32_t idx = ((x << BITWISE_NUM_BITS) | y) + (sel == 1u ? (1u << (2 * BITWISE_NUM_BITS)) : 0u);   // [range | xor]
-            if (sel <= 1u && idx < (2u << (2 * BITWISE_NUM_BITS))) hist_add(bitwise_hist, idx, m);
+            constexpr uint32_t n = 1u << BITWISE_NUM_BITS;
+            if (x < n && y < n && sel <= 1u) hist_add(bitwise_hist, ((x << BITWISE_NUM_BITS) | y) + sel * n * n, m);   // [range | xor]
         }
 #undef PB_ARG
     }
