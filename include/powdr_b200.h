@@ -45,7 +45,9 @@ int pb_ctx_synchronize(pb_ctx_t* ctx);
 /* Poseidon2 instantiation as data (canonical values): 8x16 external round constants (4 initial then 4 terminal),
  * 13 internal, 16-entry internal diagonal V (matrix 1 + diag(V)).  Default = include/pb_poseidon2_constants.h (Plonky3's
  * default BabyBear width-16 instance).  The DEVICE copy is one __constant__ bank per process and GPU: setting it on one context
- * changes the hashing of every context of this process on that GPU -- use one instantiation per process. */
+ * changes the hashing of every context of this process on that GPU -- use one instantiation per process.  pb_ctx_create puts
+ * the default back in that bank: a context that set other constants before then proves with a device that disagrees with its
+ * transcript, and its proofs end in PB_ERR_INTERNAL. */
 int pb_ctx_set_poseidon2(pb_ctx_t* ctx, const uint32_t rc_ext[8][16], const uint32_t rc_int[13], const uint32_t diag_m1[16]);
 
 /* pinned host memory + representation helpers */
@@ -99,6 +101,9 @@ int pb_merkle_commit(pb_ctx_t* ctx, const uint32_t* const* d_mats, const size_t*
 int pb_merkle_commit_rows8(pb_ctx_t* ctx, const uint32_t* d_rows, size_t log_height, uint32_t* d_digest_layers, uint32_t root_out[8]);
 /* n independent permutations of [n][16] states, in place (tests, micro-benchmarks) */
 int pb_poseidon2_permute(pb_ctx_t* ctx, uint32_t* d_states, size_t n, int reps);
+/* the same on the 16-lanes-per-permutation form that Merkle tops, short leaf sponges and the FRI challenges run on (tests,
+ * micro-benchmarks) */
+int pb_poseidon2_permute_coop(pb_ctx_t* ctx, uint32_t* d_states, size_t n);
 
 /* ---- stage 3b: FRI fold (replaces the commit-phase fold of pcs_opening; SURVEY.md §8 a9) -----------------------------
  * d_in: 2^log_len Ext4 elements [len][4], bit-reversed evaluations over shift*<w_len>; d_out: [len/2][4]. */

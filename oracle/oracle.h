@@ -29,6 +29,10 @@ void orc_lde_batch(const uint32_t* trace, unsigned log_n, size_t width, unsigned
 /* ---- Poseidon2 (width 16, x^7, 8 full + 13 partial) ---- */
 void orc_poseidon2_permute(uint32_t state[16]);
 void orc_poseidon2_permute_with(uint32_t state[16], const uint32_t* rc_ext, const uint32_t* rc_int, const uint32_t* diag);
+/* install the instantiation (canonical rc_ext [8][16], rc_int [13], diag [16]) that orc_poseidon2_permute and everything built on it
+   uses; reset: back to the default.  Process-wide: not to be changed while another thread hashes.  fast.c keeps the default. */
+void orc_set_poseidon2(const uint32_t* rc_ext, const uint32_t* rc_int, const uint32_t* diag);
+void orc_reset_poseidon2(void);
 void orc_hash_row(const uint32_t* row, size_t len, uint32_t digest[8]);     /* PaddingFreeSponge<16,8,8>: overwrite-mode absorb */
 void orc_compress(const uint32_t l[8], const uint32_t r[8], uint32_t out[8]); /* TruncatedPermutation<2,8,16> */
 

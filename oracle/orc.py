@@ -143,6 +143,18 @@ def poseidon2_permute_with(state, rc_ext, rc_int, diag):
     return s
 
 
+def set_poseidon2(rc_ext, rc_int, diag):
+    """run poseidon2_permute, hash_row, compress, merkle_commit, the challenger, prove and verify (not the AVX-512 fast paths) under
+    this instantiation (canonical rc_ext [8][16], rc_int [13], diag [16]) until reset_poseidon2; process-wide"""
+    a, b, c = _u32(rc_ext), _u32(rc_int), _u32(diag)
+    assert a.size == 128 and b.size == 13 and c.size == 16
+    lib().orc_set_poseidon2(_p(a), _p(b), _p(c))
+
+
+def reset_poseidon2():
+    lib().orc_reset_poseidon2()
+
+
 def hash_row(row):
     r = _u32(row)
     d = np.empty(8, dtype=np.uint32)

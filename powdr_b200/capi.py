@@ -15,7 +15,7 @@ EXPORTS = [
     "pb_ctx_create", "pb_ctx_destroy", "pb_ctx_synchronize", "pb_ctx_set_poseidon2", "pb_host_alloc", "pb_host_free",
     "pb_device_alloc", "pb_device_free", "pb_copy_h2d", "pb_copy_d2h", "pb_memset_zero", "pb_to_monty", "pb_from_monty",
     "pb_lde_batch", "pb_air_compile", "pb_air_free", "pb_air_is_jit", "pb_air_jit_compile_only", "pb_quotient", "pb_constraint_fold", "pb_merkle_commit",
-    "pb_merkle_commit_rows8", "pb_poseidon2_permute", "pb_fri_fold", "pb_eval_at_point", "pb_deep_quotient", "pb_prove_segment", "pb_query_words", "pb_query_segment", "pb_last_openings", "pb_last_stage_ms",
+    "pb_merkle_commit_rows8", "pb_poseidon2_permute", "pb_poseidon2_permute_coop", "pb_fri_fold", "pb_eval_at_point", "pb_deep_quotient", "pb_prove_segment", "pb_query_words", "pb_query_segment", "pb_last_openings", "pb_last_stage_ms",
     "pb_ctx_set_fri_params", "pb_air_set_interactions", "pb_air_perm_width", "pb_air_logup_compile_only", "pb_allgather_caps", "pb_bus_compile", "pb_bus_free", "pb_bus_apply",
     "pb_shard_columns", "pb_lde_shard", "pb_prove_segment_sharded", "pb_query_segment_sharded", "pb_prove_chips", "pb_prove_chips_host", "pb_chips_sizes", "pb_query_chips", "pb_host_poseidon2_permute",
     "pb_prove_chips_sharded", "pb_query_chips_sharded", "pb_ctx_set_memory_budget", "pb_last_row_blocks", "pb_footprint_bytes",
@@ -488,6 +488,18 @@ class Context:
 
     def poseidon2_permute(self, d_states_ptr, n, reps=1):
         _chk(self.lib.pb_poseidon2_permute(self.h, C.c_void_p(d_states_ptr), C.c_size_t(n), C.c_int(reps)), "pb_poseidon2_permute")
+
+    def poseidon2_permute_coop(self, d_states_ptr, n):
+        """pb_poseidon2_permute_coop: the 16-lane form of the permutation on [n][16] device states, in place"""
+        _chk(self.lib.pb_poseidon2_permute_coop(self.h, C.c_void_p(d_states_ptr), C.c_size_t(n)), "pb_poseidon2_permute_coop")
+
+    def set_poseidon2(self, rc_ext, rc_int, diag_m1):
+        """pb_ctx_set_poseidon2: canonical rc_ext [8][16], rc_int [13], diag_m1 [16].  The device constants are shared by every context
+        on the GPU, and a later Context() on it puts the default back"""
+        a, b, c = _u32(rc_ext), _u32(rc_int), _u32(diag_m1)
+        assert a.size == 128 and b.size == 13 and c.size == 16
+        _chk(self.lib.pb_ctx_set_poseidon2(self.h, a.ctypes.data_as(C.c_void_p), b.ctypes.data_as(C.c_void_p), c.ctypes.data_as(C.c_void_p)),
+             "pb_ctx_set_poseidon2")
 
     def fri_fold(self, d_in_ptr, log_len, shift, beta, d_out_ptr):
         b = (C.c_uint32 * 4)(*[int(x) for x in beta])

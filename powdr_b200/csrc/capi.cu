@@ -878,6 +878,15 @@ int pb_poseidon2_permute(pb_ctx_t* ctx, uint32_t* d_states, size_t n, int reps) 
     return 0;
 }
 
+int pb_poseidon2_permute_coop(pb_ctx_t* ctx, uint32_t* d_states, size_t n) {
+    if (!ctx || !d_states) return PB_ERR_INVALID_ARG;
+    if (!n) return 0;
+    p2::permute_states_coop_kernel<<<(unsigned)((16 * n + 255) / 256), 256, 0, ctx->stream>>>(d_states, n);
+    LAUNCHED(ctx);
+    CK(cudaGetLastError());
+    return 0;
+}
+
 // ---------------------------------------------------------------------------------------------------------------------
 // outputs [j0, j0 + n_out) of the folded codeword only when n_out != 0 (d_in / d_out then point at that block: inputs 2*j0.., outputs j0..)
 static int fri_fold_m(pb_ctx* ctx, const uint32_t* d_in, size_t log_len, uint32_t shift_m, bb::E4 beta_m, uint32_t* d_out, size_t j0 = 0,

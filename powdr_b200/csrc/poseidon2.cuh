@@ -426,4 +426,16 @@ __global__ void __launch_bounds__(256, 1) permute_states_kernel(uint32_t* states
     for (int k = 0; k < 16; k++) states[16 * i + k] = s[k];
 }
 
+// one permutation per 16-lane group on [n][16] states -- the tests' way to give permute_coop16 a whole state of their choosing.  No
+// early return: a dead group beside a live one in the last warp still takes part in the shuffles.
+__global__ void __launch_bounds__(256) permute_states_coop_kernel(uint32_t* states, size_t n) {
+    const int lane = threadIdx.x & 15;
+    const size_t i = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 4;
+    const bool live = i < n;
+    const CoopConsts k = coop_load(lane);
+    uint32_t x = live ? states[16 * i + lane] : 0u;
+    x = permute_coop16(x, lane, k);
+    if (live) states[16 * i + lane] = x;
+}
+
 }  // namespace p2

@@ -311,6 +311,7 @@ def test_entry_points_reject_null_arguments_before_touching_the_device():
     assert lib.pb_prove_segment_sharded(z, z, z, C.c_size_t(4), C.c_size_t(1), C.c_uint32(0), z, z) == INVALID
     assert lib.pb_lde_shard(z, z, C.c_size_t(6), C.c_size_t(1), C.c_uint32(31), C.c_int(2), C.c_int(0), z) == INVALID
     assert lib.pb_poseidon2_permute(z, z, n0, C.c_int(1)) == INVALID
+    assert lib.pb_poseidon2_permute_coop(z, z, n0) == INVALID
     first, count = C.c_size_t(), C.c_size_t()
     assert lib.pb_shard_columns(C.c_size_t(10), C.c_int(4), C.c_int(4), C.byref(first), C.byref(count)) == INVALID      # rank out of range
     assert lib.pb_query_words(C.c_size_t(10), C.c_size_t(3), n0, z) == INVALID
