@@ -110,10 +110,13 @@ int pb_poseidon2_permute_coop(pb_ctx_t* ctx, uint32_t* d_states, size_t n);
 int pb_fri_fold(pb_ctx_t* ctx, const uint32_t* d_in, size_t log_len, uint32_t shift, const uint32_t beta[4], uint32_t* d_out);
 
 /* ---- openings + reduced opening (the opening phase of pcs_opening; SURVEY.md §8f-4, widened in round 1) -------------------
- * pb_eval_at_point: y_k = f_k(zeta) for `width` columns given as 2^log_n evaluations over shift*H (natural order);
+ * pb_eval_at_point: y_k = f_k(zeta) for `width` columns given as 2^log_n evaluations over shift*H (natural order), f_k the
+ *   polynomial of degree < 2^log_n through them; any zeta, including a point shift*w^i of shift*H, where y_k is row i of column k.
  *   d_ys: [width][4] Ext4 values (Montgomery limbs).
  * pb_deep_quotient: ro[r] = (sum_j gamma^j (f_j[r] - y_j)) / (x_r - zeta) over the LDE domain shift*H' (bit-reversed rows),
- *   j over all columns of d_mats in order; d_ys as produced by pb_eval_at_point; d_out: [2^log_m][4]. Synchronises (reads d_ys). */
+ *   j over all columns of d_mats in order; d_ys as produced by pb_eval_at_point; d_out: [2^log_m][4]. Synchronises (reads d_ys).
+ *   zeta on shift*H' (a base-field zeta with (zeta/shift)^(2^log_m) = 1), where x_r - zeta = 0 at one row, is PB_ERR_UNSUPPORTED,
+ *   returned before any kernel is launched. */
 int pb_eval_at_point(pb_ctx_t* ctx, const uint32_t* d_mat, size_t log_n, size_t width, uint32_t shift, const uint32_t zeta[4],
                      uint32_t* d_ys);
 int pb_deep_quotient(pb_ctx_t* ctx, const uint32_t* const* d_mats, const size_t* widths, size_t n_mats, size_t log_m, uint32_t shift,

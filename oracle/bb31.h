@@ -80,4 +80,11 @@ static inline bb4_t bb4_inv(bb4_t a) {
     bb4_t s = {{i0, 0, i1, 0}};
     return bb4_mul(conj, s);
 }
+/* z lies on shift*H, |H| = 2^log_n: a base-field point with (z/shift)^(2^log_n) = 1 (canonical limbs) */
+static inline int bb4_in_coset(const uint32_t z[4], uint32_t shift, unsigned log_n) {
+    if (z[1] | z[2] | z[3]) return 0;
+    uint32_t y = bb_mul(z[0], bb_inv(shift));
+    for (unsigned i = 0; i < log_n; i++) y = bb_mul(y, y);
+    return y == 1;
+}
 #endif

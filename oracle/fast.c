@@ -486,7 +486,8 @@ static void e4m_batch_inverse(bb4_t* d, size_t n) {
 
 void orcf_eval_at_point(const uint32_t* mat, unsigned log_n, size_t width, uint32_t shift, const uint32_t zeta[4], uint32_t* out) {
     const size_t n = (size_t)1 << log_n;
-    if (n < 16) { orc_eval_at_point(mat, log_n, width, shift, zeta, out); return; }
+    /* below 16 rows, and at a point of the domain, where one weight's denominator is 0: the scalar restatement */
+    if (n < 16 || bb4_in_coset(zeta, shift, log_n)) { orc_eval_at_point(mat, log_n, width, shift, zeta, out); return; }
     bb4_t z = {{zeta[0], zeta[1], zeta[2], zeta[3]}};
     z = bb4_scale(z, bb_inv(shift));
     /* weights w^i / (z - w^i), Montgomery limbs, SoA */
@@ -613,9 +614,10 @@ void orcf_deep_quotient_groups(const uint32_t* const* cols, const uint32_t* grou
     free(gp); free(ysum); free(acc_all); free(den);
 }
 
-/* drop-in for orc_deep_quotient (one point, all matrices) */
-void orcf_deep_quotient(const uint32_t* const* mats, const size_t* widths, size_t n_mats, unsigned log_m, uint32_t shift,
-                        const uint32_t zeta[4], const uint32_t gamma[4], const uint32_t* ys, uint32_t* out) {
+/* drop-in for orc_deep_quotient (one point, all matrices), with its refusal of a zeta on shift*H' */
+int orcf_deep_quotient(const uint32_t* const* mats, const size_t* widths, size_t n_mats, unsigned log_m, uint32_t shift,
+                       const uint32_t zeta[4], const uint32_t gamma[4], const uint32_t* ys, uint32_t* out) {
+    if (bb4_in_coset(zeta, shift, log_m)) return -1;
     const size_t m = (size_t)1 << log_m;
     size_t total = 0;
     for (size_t i = 0; i < n_mats; i++) total += widths[i];
@@ -629,6 +631,7 @@ void orcf_deep_quotient(const uint32_t* const* mats, const size_t* widths, size_
     for (size_t j = 0; j < total; j++) { memcpy(gp + 4 * j, cur.c, 16); cur = bb4_mul(cur, g); }
     orcf_deep_quotient_groups(cols, grp, total, zeta, 1, log_m, shift, gp, ys, out);
     free(cols); free(grp); free(gp);
+    return 0;
 }
 
 /* =====================================================================================================================

@@ -131,9 +131,11 @@ void orc_eval_at_point(const uint32_t* mat, unsigned log_n, size_t width, uint32
 
 /* reduced opening at one point over the LDE domain shift*H' (bit-reversed rows):
    ro[r] = ( sum_j gamma^j * (f_j[r] - y_j) ) / (x_r - zeta),   x_r = shift * w_m^{bitrev(r)},  j runs over all columns of all
-   matrices in order.  mats: column-major, height m = 2^log_m.  ys: [total_width][4].  out: [m][4]. */
-void orc_deep_quotient(const uint32_t* const* mats, const size_t* widths, size_t n_mats, unsigned log_m, uint32_t shift,
-                       const uint32_t zeta[4], const uint32_t gamma[4], const uint32_t* ys, uint32_t* out) {
+   matrices in order.  mats: column-major, height m = 2^log_m.  ys: [total_width][4].  out: [m][4].
+   Returns -1, and writes nothing, when zeta lies on shift*H' (x_r - zeta has no inverse at one row). */
+int orc_deep_quotient(const uint32_t* const* mats, const size_t* widths, size_t n_mats, unsigned log_m, uint32_t shift,
+                      const uint32_t zeta[4], const uint32_t gamma[4], const uint32_t* ys, uint32_t* out) {
+    if (bb4_in_coset(zeta, shift, log_m)) return -1;
     size_t m = (size_t)1 << log_m, total = 0;
     for (size_t i = 0; i < n_mats; i++) total += widths[i];
     bb4_t g = {{gamma[0], gamma[1], gamma[2], gamma[3]}}, z = {{zeta[0], zeta[1], zeta[2], zeta[3]}};
@@ -161,6 +163,7 @@ void orc_deep_quotient(const uint32_t* const* mats, const size_t* widths, size_t
         memcpy(out + 4 * (size_t)r, v.c, 16);
     }
     free(gp);
+    return 0;
 }
 
 /* reduced opening over several (column group, point) pairs:

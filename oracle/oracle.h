@@ -64,8 +64,9 @@ void orc_fri_fold(const uint32_t* in, unsigned log_len, uint32_t shift, const ui
 
 /* ---- openings + DEEP reduced opening (row f-4 of SURVEY.md §8, widened in round 1) ---- */
 void orc_eval_at_point(const uint32_t* mat, unsigned log_n, size_t width, uint32_t shift, const uint32_t zeta[4], uint32_t* out);
-void orc_deep_quotient(const uint32_t* const* mats, const size_t* widths, size_t n_mats, unsigned log_m, uint32_t shift,
-                       const uint32_t zeta[4], const uint32_t gamma[4], const uint32_t* ys, uint32_t* out);
+/* -1 (nothing written) when zeta lies on the LDE domain shift*H' */
+int orc_deep_quotient(const uint32_t* const* mats, const size_t* widths, size_t n_mats, unsigned log_m, uint32_t shift,
+                      const uint32_t zeta[4], const uint32_t gamma[4], const uint32_t* ys, uint32_t* out);
 
 /* ---- DuplexChallenger<BabyBear, Perm16, 16, 8> ---- */
 typedef struct { uint32_t sponge[16]; uint32_t in_buf[8]; int n_in; uint32_t out_buf[8]; int n_out; } orc_challenger_t;
@@ -153,8 +154,8 @@ void orcf_constraint_fold(const uint32_t* bc, const orc_span_t* spans, size_t n_
 void orcf_quotient(const uint32_t* bc, const orc_span_t* spans, size_t n_constraints, const uint32_t* lde, unsigned log_n,
                    unsigned log_blowup, uint32_t shift, const uint32_t alpha[4], uint32_t* quotient);
 void orcf_eval_at_point(const uint32_t* mat, unsigned log_n, size_t width, uint32_t shift, const uint32_t zeta[4], uint32_t* out);
-void orcf_deep_quotient(const uint32_t* const* mats, const size_t* widths, size_t n_mats, unsigned log_m, uint32_t shift,
-                        const uint32_t zeta[4], const uint32_t gamma[4], const uint32_t* ys, uint32_t* out);
+int orcf_deep_quotient(const uint32_t* const* mats, const size_t* widths, size_t n_mats, unsigned log_m, uint32_t shift,
+                       const uint32_t zeta[4], const uint32_t gamma[4], const uint32_t* ys, uint32_t* out);
 void orcf_logup_perm_trace(const uint32_t* trace, unsigned log_n, const uint32_t* ibc, const orc_span_t* isp, const orc_interaction_t* ints,
                            size_t n_ints, const uint32_t* chunk_start, size_t n_chunks, const uint32_t alpha_lu[4], const uint32_t beta_lu[4],
                            uint32_t* perm, uint32_t cumsum[4]);

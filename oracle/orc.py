@@ -226,14 +226,16 @@ def eval_at_point(mat, shift, zeta):
 
 
 def deep_quotient(mats, shift, zeta, gamma, ys):
-    """mats: list of (width_i, m) column-major LDE matrices (bit-reversed rows over shift*H'); ys: (sum width, 4) -> (m, 4)"""
+    """mats: list of (width_i, m) column-major LDE matrices (bit-reversed rows over shift*H'); ys: (sum width, 4) -> (m, 4).
+    ValueError when zeta lies on shift*H'."""
     mats = [_u32(x) for x in mats]
     m = mats[0].shape[1]
     ptrs = (C.c_void_p * len(mats))(*[x.ctypes.data for x in mats])
     widths = (C.c_size_t * len(mats))(*[x.shape[0] for x in mats])
     z, g, y = _u32(zeta), _u32(gamma), _u32(ys)
     out = np.empty((m, 4), dtype=np.uint32)
-    lib().orc_deep_quotient(ptrs, widths, C.c_size_t(len(mats)), C.c_uint(m.bit_length() - 1), C.c_uint32(shift), _p(z), _p(g), _p(y), _p(out))
+    if lib().orc_deep_quotient(ptrs, widths, C.c_size_t(len(mats)), C.c_uint(m.bit_length() - 1), C.c_uint32(shift), _p(z), _p(g), _p(y), _p(out)):
+        raise ValueError("zeta lies on the LDE domain: the reduced opening has no value at one row")
     return out
 
 
@@ -388,7 +390,8 @@ def fast_deep_quotient(mats, shift, zeta, gamma, ys):
     widths = (C.c_size_t * len(mats))(*[x.shape[0] for x in mats])
     z, g, y = _u32(zeta), _u32(gamma), _u32(ys)
     out = np.empty((m, 4), dtype=np.uint32)
-    lib().orcf_deep_quotient(ptrs, widths, C.c_size_t(len(mats)), C.c_uint(m.bit_length() - 1), C.c_uint32(shift), _p(z), _p(g), _p(y), _p(out))
+    if lib().orcf_deep_quotient(ptrs, widths, C.c_size_t(len(mats)), C.c_uint(m.bit_length() - 1), C.c_uint32(shift), _p(z), _p(g), _p(y), _p(out)):
+        raise ValueError("zeta lies on the LDE domain: the reduced opening has no value at one row")
     return out
 
 

@@ -977,7 +977,15 @@ static int fri_commit_phase(pb_ctx* ctx, Challenger& ch, uint32_t layer0, size_t
 
 // ---------------------------------------------------------------------------------------------------------------------
 static int eval_weighted_m(pb_ctx* ctx, const uint32_t* d_mat, size_t N, size_t width, bb::E4 pref, uint32_t* d_ys);
-// openings: y_k = f_k(zeta) for columns given as evaluations over shift*H (natural order); d_ys: [width][4] Montgomery
+// z (Montgomery) lies on shift*H, |H| = 2^log_n: a base-field point with (z/shift)^(2^log_n) = 1
+static bool on_coset_m(bb::E4 z_m, uint32_t shift_m, size_t log_n) {
+    if (z_m.c[1] | z_m.c[2] | z_m.c[3]) return false;
+    uint32_t y = bb::mul(z_m.c[0], bb::inv(shift_m));
+    for (size_t i = 0; i < log_n; i++) y = bb::mul(y, y);
+    return y == bb::R1;
+}
+// openings: y_k = f_k(zeta) for columns given as evaluations over shift*H (natural order); d_ys: [width][4] Montgomery.
+// Any zeta: at a point shift*w^i of the domain itself y_k is row i of column k.
 static int eval_at_point_m(pb_ctx* ctx, const uint32_t* d_mat, size_t log_n, size_t width, uint32_t shift_m, bb::E4 zeta_m, uint32_t* d_ys) {
     const size_t N = (size_t)1 << log_n;
     if (width == 0) return 0;
@@ -985,8 +993,11 @@ static int eval_at_point_m(pb_ctx* ctx, const uint32_t* d_mat, size_t log_n, siz
     if (rc) return rc;
     // f(zeta) = g(zeta/shift) with g's evaluations over H:  g(z) = (z^N - 1)/N * sum_i g_i * w^i / (z - w^i)
     const bb::E4 z = bb::e4_scale(zeta_m, bb::inv(shift_m));
-    deep::bary_weights_kernel<<<(unsigned)((N + 255) / 256), 256, 0, ctx->stream>>>(ctx->ws_w.p, (int)log_n, h_root_of_unity_m((int)log_n), z);
+    const bool on_domain = on_coset_m(zeta_m, shift_m, log_n);        // z = w^i: one-hot weights, prefactor 1
+    deep::bary_weights_kernel<<<(unsigned)((N + 255) / 256), 256, 0, ctx->stream>>>(ctx->ws_w.p, (int)log_n, h_root_of_unity_m((int)log_n), z,
+                                                                                    on_domain ? 1 : 0);
     LAUNCHED(ctx);
+    if (on_domain) return eval_weighted_m(ctx, d_mat, N, width, bb::E4{{bb::R1, 0u, 0u, 0u}}, d_ys);
     bb::E4 zn = z;
     for (size_t i = 0; i < log_n; i++) zn = bb::e4_mul(zn, zn);
     zn.c[0] = bb::sub(zn.c[0], bb::R1);
@@ -1015,12 +1026,15 @@ static int eval_weighted_m(pb_ctx* ctx, const uint32_t* d_mat, size_t N, size_t 
 // Columns of group 0 go in runs of equal stride; a run of group-1 columns that repeats a group-0 run (same base, stride, count: the
 // permutation trace opened at zeta and at zeta*w) is attached to it, so those columns are read from HBM once.  One launch per
 // DQ_MAX_SEGS runs: the first writes d_out, the later ones add to it.
+// A point on the domain shift*H' (x_r - z has no inverse at one row) is PB_ERR_UNSUPPORTED, before anything is launched.
 static int deep_quotient_groups_m(pb_ctx* ctx, const std::vector<const uint32_t*>& cols, const std::vector<uint32_t>& grp, const std::vector<uint32_t>& e,
                                   const std::vector<bb::E4>& zs, size_t log_m, uint32_t shift_m, bb::E4 gamma_m, const uint32_t* ys_m, uint32_t* d_out,
                                   size_t row0 = 0, size_t n_rows = 0) {
     const size_t n_cols = cols.size(), M = n_rows ? n_rows : (size_t)1 << log_m;
     if (n_cols == 0 || grp.size() != n_cols || e.size() != n_cols || zs.empty()) return PB_ERR_INVALID_ARG;
     if (zs.size() > 2) return PB_ERR_UNSUPPORTED;
+    for (const bb::E4& z : zs)
+        if (on_coset_m(z, shift_m, log_m)) return PB_ERR_UNSUPPORTED;
     std::vector<bb::E4> gp(n_cols);                   // gamma^e[j]: one product along a run of consecutive exponents
     std::vector<uint4> gs(n_cols);
     for (size_t j = 0; j < n_cols; j++) {

@@ -27,11 +27,17 @@ __device__ __forceinline__ bb::E4 e4_inv(bb::E4 a) {
     return bb::e4_mul(conj, s);
 }
 
-// barycentric weights over the subgroup H of size 2^log_n at the point z:  w_i = omega^i / (z - omega^i)
-__global__ void __launch_bounds__(256) bary_weights_kernel(uint4* __restrict__ w, int log_n, uint32_t omega_m, bb::E4 z) {
+// barycentric weights over the subgroup H of size 2^log_n at the point z:  w_i = omega^i / (z - omega^i).
+// one_hot (z is a point of H, where one denominator is 0 and the prefactor (z^N - 1)/N too): w_i = [omega^i == z], so that
+// with prefactor 1 the weighted sum is the value at that row.
+__global__ void __launch_bounds__(256) bary_weights_kernel(uint4* __restrict__ w, int log_n, uint32_t omega_m, bb::E4 z, int one_hot) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= ((size_t)1 << log_n)) return;
     const uint32_t x = bb::pow(omega_m, i);
+    if (one_hot) {
+        w[i] = make_uint4(x == z.c[0] ? bb::R1 : 0u, 0u, 0u, 0u);
+        return;
+    }
     bb::E4 d = z;
     d.c[0] = bb::sub(d.c[0], x);
     bb::E4 r = bb::e4_scale(e4_inv(d), x);
